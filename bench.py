@@ -19,7 +19,7 @@ A bench "step" = TICKS_PER_STEP consecutive group-ticks of every group: one fuse
 the block-table window moves up, so an engine runs indefinitely -- no reset anywhere in this
 file), and the drain of the step's Instruction stream (jr_fsm_records_async: count + scan +
 pack on the engine stream, DMA to pinned host memory on the copy stream).  L2 is flushed
-between timed steps (the working set is smaller than the 126 MB L2).  Device time is taken
+between timed steps, so no step starts with the previous one's data in the 50 MB L2.  Device time is taken
 with CUDA events on the engine's stream, per step, flush excluded; max over ranks.
 
 Arms:
@@ -202,11 +202,22 @@ class ClockSampler:
                 "reasons": reasons, "samples": len(sm), "sampled": where}
 
 
+def gpu_card(index):
+    """Name, power limit and top SM clock of the card: part of every number this run reports."""
+    try:
+        out = subprocess.check_output(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm",
+                                       "--format=csv,noheader"], text=True, stderr=subprocess.DEVNULL).strip()
+        name, power, clock = [x.strip() for x in out.split(",")][:3]
+        return {"name": name, "power_limit": power, "sm_max_clock": clock}
+    except (OSError, ValueError, subprocess.CalledProcessError):
+        return {"name": None, "power_limit": None, "sm_max_clock": None}
+
+
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, torch copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not a measured peak)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -267,8 +278,9 @@ def cpu_cluster(G, R, threads, chain_window=CHAIN_WINDOW, heartbeat_ms=100, seed
 
 def best_cpu_threads(R, cores):
     """The restatement allocates heavily; more threads than the allocator / cgroup can feed makes it SLOWER.
-    Probe a few counts on a small sample, once per host (cached under /tmp), and keep the fastest."""
-    cache = f"/tmp/josefine_b200_cpu_threads_{cores}_{R}.json"
+    Probe a few counts on a small sample, once per host (cached in the temporary directory), and keep the fastest."""
+    import tempfile
+    cache = os.path.join(tempfile.gettempdir(), f"josefine_b200_cpu_threads_{cores}_{R}.json")
     try:
         return int(json.load(open(cache))["threads"])
     except (OSError, ValueError, KeyError):
@@ -346,6 +358,40 @@ def run_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------
+# --dump-outputs: what the timed path computed, for comparing two builds output for output
+
+DUMP_RECORD_ROWS = 1 << 19      # 10 float64 = 80 B per row: 40 MiB; a larger batch is sampled (fixed seed)
+RECORD_COLUMNS = ["group", "kind", "node", "count", "id0", "addr", "tok0_lo", "tok0_hi", "stride_lo", "stride_hi"]
+
+
+def record_arrays(ptr, n):
+    """The jr_fsm_record batch at `ptr` as a [n, 10] float64 array (RECORD_COLUMNS; u64 fields split into exact u32 halves)."""
+    import numpy as np
+    dt = np.dtype([("group", "<u4"), ("hdr", "<u4"), ("id0", "<u4"), ("addr", "<u4"), ("tok0", "<u8"), ("stride", "<u8")])
+    if n == 0:
+        return np.zeros((0, len(RECORD_COLUMNS)), dtype=np.float64)
+    raw = np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_uint8)), shape=(n * dt.itemsize,)).view(dt)
+    lo, hi = np.uint64(0xFFFFFFFF), np.uint64(32)
+    cols = [raw["group"], raw["hdr"] & 3, ((raw["hdr"] >> 2) & 7) + 1, raw["hdr"] >> 8, raw["id0"], raw["addr"],
+            raw["tok0"] & lo, raw["tok0"] >> hi, raw["stride"] & lo, raw["stride"] >> hi]
+    return np.stack([c.astype(np.float64) for c in cols], axis=1)
+
+
+def dump_outputs(out_dir, table, records):
+    """leader_table.npy: [G, 3] (term, leader id, commit) per group, what jr_leader_table returns after the last step;
+    fsm_records.npy: that step's Instruction records (see record_arrays), in the order the drain delivered them, or a
+    fixed, seeded sample of rows in that order when there are more than DUMP_RECORD_ROWS."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "leader_table.npy"), np.array(table, dtype=np.float64).reshape(-1, 3))
+    if records is not None:
+        if len(records) > DUMP_RECORD_ROWS:
+            keep = np.sort(np.random.default_rng(SEED).choice(len(records), DUMP_RECORD_ROWS, replace=False))
+            records = records[keep]
+        np.save(os.path.join(out_dir, "fsm_records.npy"), records)
+
+
+# ---------------------------------------------------------------------------------------------
 # GPU arms
 
 class Bench:
@@ -364,7 +410,7 @@ class Bench:
         torch.cuda.set_device(self.local)
         if self.world > 1:
             # The 1 MB announce runs next to the step's drain kernels, never next to sym2_kernel (one_step below).
-            # (NCCL's own channel count: capped at 2 the 2 x 1 MB all-gather took 134 us, at 1 channel 255 us)
+            # NCCL keeps its own channel count.
             dist.init_process_group("nccl", device_id=torch.device("cuda", self.local))
         global FOLD_THREADS
         if FOLD_THREADS <= 0:     # the box's cgroup may allow far fewer cores than it shows, and the fold pool's workers spin between two
@@ -405,7 +451,7 @@ class Bench:
         return float(t.item())
 
     # ---- device-resident: proposals generated in the kernel, Instruction stream drained every step
-    def device_resident(self, G, R, steps, warmup, announce=True, sampler=None, **eng_kw):
+    def device_resident(self, G, R, steps, warmup, announce=True, sampler=None, dump_dir=None, **eng_kw):
         torch, dist = self.torch, self.dist
         S = TICKS_PER_STEP
         capture = os.environ.get("JR_BENCH_CAPTURE", "1") != "0"      # diagnostic A/B only; the reported runs capture
@@ -420,6 +466,7 @@ class Bench:
         totals = (C.c_uint64 * 3)()
         applied = (C.c_uint32 * (G * R))()
         outstanding = [0]
+        keep = [False, None]      # [copy the batches taken from now on, the last one copied]
 
         def take():
             # device-resident leg: the batch must have LANDED in pinned host memory, but it is not walked here (the
@@ -427,6 +474,8 @@ class Bench:
             ptr, batch = C.POINTER(abi.FsmRecord)(), abi.FsmBatch()
             st = lib.jr_fsm_records_wait(h, C.byref(ptr), C.byref(batch))
             assert st == 0, (st, batch.n_dropped)
+            if keep[0]:
+                keep[1] = record_arrays(ptr, batch.n_records)
             totals[0] += batch.n_instructions
             totals[2] += batch.n_records
             outstanding[0] -= 1
@@ -434,8 +483,8 @@ class Bench:
         def one_step():
             if world > 1 and announce and announce_done[0] is not None:
                 # The previous announce must be over before the fused run starts: `leaders` is rewritten below, and sym2_kernel
-                # needs 1,024 of the GPU's 1,036 CTA slots in ONE wave -- an NCCL kernel still holding two SMs would push CTAs
-                # into a second wave and stretch the step by the collective's duration.
+                # keeps every SM busy for the whole run -- an NCCL kernel still holding two SMs would delay CTAs behind it and
+                # stretch the step by the collective's duration.
                 self.stream.wait_event(announce_done[0])
             eng.run(now[0], DT_MS, S, 1)          # (ends with jr_truncate: jr_set_auto_truncate)
             now[0] += DT_MS * S
@@ -478,6 +527,7 @@ class Bench:
                 self.stream.wait_event(announce_done[0])            # the last announce is not hidden by a next step: time it
             b.record(self.stream)
             evs.append((a, b))
+        keep[0] = dump_dir is not None        # the last batch taken below is the last timed step's
         while outstanding[0]:
             take()
         self.barrier()
@@ -488,6 +538,8 @@ class Bench:
         table = eng.leader_table()
         commit_min = min(c for (_, _, c) in table)
         assert faults == 0, f"{faults} replicas faulted during the timed region"
+        if dump_dir is not None:
+            dump_outputs(dump_dir, table, keep[1] if capture else None)
         collective_us = None
         if world > 1 and announce:          # the collective alone, no kernel next to it
             cev = []
@@ -648,7 +700,7 @@ class Bench:
                "d2h_bytes_per_step": G * 16 + (rec_bytes[0] // steps if with_output else 0), "ms_per_step": dt * 1e3 / steps,
                "commit_last": checks[-1], "faulted_replicas": faults,
                "timing": "host wall clock around all timed steps incl. the final sync, max over ranks",
-               "l2": "steps run back to back, no flush in between: one step moves ~0.4 GB through DRAM (profiles/, ncu), more than the 126 MB L2"}
+               "l2": "steps run back to back, no flush in between"}
         if trace is not None:
             out["host_ms_per_step"] = {k: v * 1e3 / steps for k, v in trace.items()}      # timed steps only
         if with_output:
@@ -692,7 +744,7 @@ class Bench:
                             "proposals/group, 256 ticks (3 fused launches)", "groups": G, "replicas": R, "ticks": 256,
                 "ms_per_trace": ms, "value": G * 256 / (ms * 1e-3), "unit": UNIT, "groups_with_leader": leaders,
                 "faulted_replicas": eng.fault_count(),
-                "note": "32 CTAs on 148 SMs: this size measures launch + per-tick latency, not throughput"}
+                "note": "32 CTAs on 132 SMs: this size measures launch + per-tick latency, not throughput"}
 
     # ---- BASELINE config #5: 65,536 x 7, 10% of the groups lose their leader every 100 ticks, compact every 256
     def config5(self, steps, warmup):
@@ -805,6 +857,7 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-others", action="store_true", help="skip configs #2/#4/#5 and the variants")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the headline's last timed step computed to DIR/*.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -819,7 +872,8 @@ def main():
         sampler.start()
 
     # ---------------- headline: config #3, device resident ----------------
-    main_res = bn.device_resident(G, R, args.steps, max(args.warmup, 20), sampler=sampler)   # >= 20 untimed steps: also nvidia-smi's start-up
+    main_res = bn.device_resident(G, R, args.steps, max(args.warmup, 20), sampler=sampler,
+                                  dump_dir=args.dump_outputs if rank == 0 else None)   # >= 20 untimed steps: also nvidia-smi's start-up
     clocks = main_res.pop("clocks")
     value, ms = main_res["value"], main_res["ms_total"]
     launches = args.steps * (6 + (1 if world > 1 else 0))   # sym2_kernel, step_kernel, truncate_kernel, fsm count / scan / pack (+ leader_table_kernel); the copy-out is a DMA
@@ -911,7 +965,7 @@ def main():
                    "parallelism": f"groups sharded over {world} GPU(s); leader-announce all_gather once per step" if world > 1
                    else "single GPU", "faulted_replicas": main_res["faulted_replicas"], "commit_min": main_res["commit_min"],
                    "untimed_steps_before_timing": max(args.warmup, 20), "host_placement": bn.placement},
-        "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e, "e2e_dense_input": e2e_dense, "e2e_no_output": e2e_plain, "gpu_launches": launches, "clocks": clocks,
+        "gpu": gpu_card(bn.local), "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e, "e2e_dense_input": e2e_dense, "e2e_no_output": e2e_plain, "gpu_launches": launches, "clocks": clocks,
         "collective_us": main_res["collective_us"], "instructions_per_step": main_res["instructions"] // args.steps,
         "other_configs": others, "variants": variants, "parity": parity,
     }

@@ -1,5 +1,5 @@
 /*
- * josefine_raft_abi.h -- C ABI of the B200 batched Chained-Raft engine.
+ * josefine_raft_abi.h -- C ABI of the H100 batched Chained-Raft engine.
  *
  * This is the drop-in boundary for josefine's Raft step path.  Every entry
  * point names the reference interface it stands in for (paths are relative to

@@ -1,7 +1,7 @@
-"""josefine_b200 -- B200-native batched Chained-Raft engine behind josefine's Raft step API.
+"""josefine_b200 -- H100-native batched Chained-Raft engine behind josefine's Raft step API.
 
 Only the hot path of tychedelia/josefine's src/raft (SURVEY.md section 8) lives
-here: csrc/ holds the sm_100a kernels and the C ABI (include/josefine_raft_abi.h),
+here: csrc/ holds the sm_90a kernels and the C ABI (include/josefine_raft_abi.h),
 raft.py the host-side mirror of the reference's Command / Apply interface.
 """
 from . import abi  # noqa: F401

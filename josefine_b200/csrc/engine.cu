@@ -1,6 +1,6 @@
-// engine.cu -- kernels + C ABI of the B200 batched Chained-Raft engine.
+// engine.cu -- kernels + C ABI of the H100 batched Chained-Raft engine.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a (see __graft_entry__.build).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a (see __graft_entry__.build).
 // No CPU fallback: without a CUDA device jr_engine_create returns JR_E_NO_DEVICE.
 //
 // Reference interfaces replaced are cited in include/josefine_raft_abi.h; the
@@ -37,7 +37,7 @@ using namespace jr;
 // ticket, in launch order, so all part k-1 tasks are running or done before any part k task starts; a part k
 // task waits for its block's part k-1 (release/acquire on d.done[block]) and then continues from the state
 // and mailboxes that task stored -- exactly what the next launch would do.  The point is the last wave:
-// 2048 equal tasks on 592 CTA slots take 4 rounds, 4096 half-length tasks take 7 half-rounds.
+// 600 equal tasks on 528 CTA slots (132 SMs x 4) take 2 rounds, 1200 half-length tasks take 3 half-rounds.
 #ifdef JR_EMU
 #ifdef JR_EMU_BREAK_HANDOFF  // negative control of tests/emu/tsan_split.cpp: the race detector must notice this
 #define JR_EMU_HANDOFF_ACQUIRE __ATOMIC_RELAXED
@@ -744,6 +744,7 @@ struct jr_engine {
   int force_sorted = 0;      // JR_STEP_VARIANT=sorted|plain pins the kernel variant (tests, A/B)
   uint64_t launches_sorted = 0, launches_total = 0, launches_split = 0;
   uint32_t slots = 0;        // CTAs of the step kernel the device holds at once (occupancy x SMs)
+  uint32_t sms = 0;          // SMs of the device
   uint32_t force_parts = 0;  // JR_PARTS=n pins the split (tests, A/B); 0 = choose_parts
   int cur = 0;               // outbox index the NEXT step writes
   uint64_t step_index = 0;
@@ -1130,6 +1131,7 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
       DISPATCH_R(d.R, (aerr = step_occupancy_r<RR>(&per_sm, smem)));
       if (aerr == cudaSuccess) aerr = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
       e->slots = (uint32_t)(per_sm * sms);
+      e->sms = (uint32_t)sms;
     }
 #endif
     if (const char* ev = getenv("JR_STEP_VARIANT")) e->force_sorted = !strcmp(ev, "sorted") ? 1 : (!strcmp(ev, "plain") ? -1 : 0);
@@ -1342,8 +1344,8 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
   } else {
     // Copy engine, speculatively: the batch size is only known on the device, so copy as many records as the previous
     // batch held plus a margin; fsm_records_take fetches the rest in the (rare) case the batch turned out larger.
-    // (fsm_copy_kernel's stores to host memory share LSUs with the next step's kernel: one wave of CTAs, so the
-    // slowest SM sets its duration.  A DMA copy takes nothing from the SMs.)
+    // (fsm_copy_kernel's stores to host memory share LSUs with the next step's kernel: every SM runs equal
+    // CTAs, so the slowest SM sets its duration.  A DMA copy takes nothing from the SMs.)
     const size_t guess = std::min<size_t>(e->fsm_cap, std::max<size_t>(last_records + last_records / 8 + 1024, 16384));
     if (guess) CK(cudaMemcpyAsync(e->fsm_host[b], e->fsm_stage[b], guess * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
     CK(cudaMemcpyAsync(e->fsm_host_hdr[b], e->fsm_stage_hdr[b], sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
@@ -1645,7 +1647,7 @@ jr_status jr_run_tokens(jr_engine* e, uint64_t now0, uint32_t dt, uint32_t n_ste
   CK(cudaEventRecord(e->batch_ready[b], e->h2d));
   CK(cudaStreamWaitEvent(e->stream, e->batch_ready[b], 0));
   // on the engine stream: ordered after the leader_table_kernel that last wrote `route`
-  const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)148 * 16);
+  const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)std::max(e->sms, 1u) * 16);
   JR_LAUNCH(route_tokens_kernel, blocks, 256, e->stream, e->tokbuf[b], e->route, e->batch[b], G, n);
   CK(cudaGetLastError());
   return batch_launch(e, b, now0, dt, n_steps);

@@ -1,4 +1,4 @@
-// raft_device.cuh -- device-side Chained-Raft replica state machine (sm_100a).
+// raft_device.cuh -- device-side Chained-Raft replica state machine (sm_90a).
 //
 // One lane owns one replica.  A CTA is GROUPS_PER_CTA(=32) consecutive groups x R
 // replicas; warp w holds replica index w of those 32 groups, so every state

@@ -51,7 +51,7 @@ struct SymMail {
 // table, the followers' identical tables) of SYM_ROWS entries {id, next, token}, laid out [cache][slot][lane] so that a
 // lane's access is one conflict-free 128-bit LDS/STS.  Everything a steady group reads was written a few ticks ago, so
 // after the fill at entry no table READ leaves the SM (rows are still written through to HBM).  (A register shift
-// register cost ~400 instructions per tick in compare/select chains; local-memory arrays were slower still.)
+// register costs compare/select chains every tick; local-memory arrays were slower still.)
 constexpr uint32_t SYM_ROWS = 8;
 #ifndef JR_SYM_LANES
 #define JR_SYM_LANES 128   // (A/B builds override it)
@@ -518,7 +518,7 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, SPLIT>& s, SymMail& m, con
   s.flo = lo;
   const uint64_t grow = (uint64_t)p.n_ticks * (1u + p.n_synth) + 2u;
   if ((uint64_t)s.maxkey + grow >= (uint64_t)s.tbase + d.cap || (uint64_t)s.maxkey + grow >= FS_NOTIFY_BIT) return false;
-  {  // batches of independent loads, no exit in between: the latency of ~100 dependent loads was 14% of the kernel
+  {  // batches of independent loads, no exit in between: one dependent load at a time would serialise ~100 latencies
     constexpr uint32_t B = 4;
     bool same = true;
     for (uint32_t b0 = lo; b0 <= s.fmaxkey && same; b0 += B) {
@@ -798,8 +798,11 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
 // planes and outbox, the follower lane those of the followers.  Either side may abort: it says so in its mail, the
 // other side sees it one barrier later, and after the last barrier both check the other's final mail, so a group is
 // either left (by both) or not at all.
+// CTAs per SM the register allocation must allow.  The shared memory (480 B per group) caps an SM at 7 CTAs = 448 groups, so
+// on 132 SMs 65,536 groups take two waves whatever the register budget; 4 CTAs (128 registers, next to no spills) run the
+// two waves faster than 7 (72 registers, spilling) run one and a bit.
 #ifndef JR_SYM2_MINCTAS
-#define JR_SYM2_MINCTAS 7
+#define JR_SYM2_MINCTAS 4
 #endif
 #ifndef JR_SYM2_ROLES
 #define JR_SYM2_ROLES 3   // (register-need experiments: 1 = leader code only, 2 = follower code only)
@@ -808,7 +811,7 @@ template <int R>
 __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(const Dev d, const StepParams p, uint8_t* symdone, uint8_t* symblk) {
   JR_DYN_SMEM(uint4, smem);
   // One __syncthreads() per tick for both warp pairs of the CTA.  (A named barrier per pair -- `bar.sync 0/1, 64`, the
-  // pairs never need each other -- measured 3% SLOWER, twice; with a register operand for the id ptxas charges the CTA
+  // pairs never need each other -- was slower; with a register operand for the id ptxas charges the CTA
   // all 16 barriers and only one CTA fits an SM.)
   auto pair_sync = [] { __syncthreads(); };
   constexpr uint32_t S = SYM2_GROUPS;

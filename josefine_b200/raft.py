@@ -581,7 +581,7 @@ def load_engine_library() -> C.CDLL:
 
 
 class RaftEngine(RaftApi):
-    """G x R Raft replicas resident in one B200's HBM, stepped by the sm_100a kernels."""
+    """G x R Raft replicas resident in one H100's HBM, stepped by the sm_90a kernels."""
 
     def __init__(self, cfg: abi.Config):
         lib = load_engine_library()

@@ -58,9 +58,9 @@ def test_election_timeout_is_the_same_function_everywhere(engine_lib, oracle_lib
             oracle_lib.jro_election_timeout(seed, g, n, d, 500, 1000)
 
 
-def test_engine_library_is_sm100a_cuda(engine_lib):
+def test_engine_library_is_sm90a_cuda(engine_lib):
     out = subprocess.run(["cuobjdump", "-lelf", ENGINE_LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out
+    assert "sm_90a" in out, out
 
 
 def test_create_without_gpu_fails_loudly(engine_lib):

@@ -1,5 +1,5 @@
 """GPU suite: the CUDA engine, called through the C ABI (libjosefine_b200.so),
-against the C++ restatement oracle -- bit for bit.  Needs a B200."""
+against the C++ restatement oracle -- bit for bit.  Needs an H100."""
 import pytest
 
 from josefine_b200 import abi, RaftEngine

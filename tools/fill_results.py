@@ -3,7 +3,7 @@
 
 usage: fill_results.py <bench.json> [<profile_note.txt>]
 Rewrites the text between `<!-- results:begin -->` / `<!-- results:end -->` in BASELINE.md and DESIGN.md.
-Pure formatting: every number printed comes from the JSON (a bench.py run on a B200, never under a profiler)."""
+Pure formatting: every number printed comes from the JSON (a bench.py run on an H100, never under a profiler)."""
 import json
 import os
 import re
@@ -48,10 +48,12 @@ def table(d):
         rows.append(f"| #3, C++ restatement of src/raft on the host (NOT josefine) | same step, {cpu['cores']} threads / 1 thread | {sci(cpu['value'])} / {sci(cpu.get('value_1_thread'))} | - |")
     out = "\n".join(rows)
     out += (f"\n\nRoofline of the headline line (`roofline` in the JSON): {rf['algorithmic_bytes_per_group_tick']:.0f} B per group-tick in the reference's "
-            f"widths -> {rf['achieved']:.0f} GB/s = **{rf['frac']:.2f}** of the measured HBM peak ({rf['peak']:.0f} GB/s); in this engine's wider "
+            f"widths -> {rf['achieved']:.0f} GB/s = **{rf['frac']:.2f}** of the HBM peak ({rf['peak']:.0f} GB/s, {rf['peak_source']}); in this engine's wider "
             f"layout {rf['layout_bytes_per_group_tick']:.0f} B -> {rf['frac_layout']:.2f}; real DRAM traffic of the dominant kernel "
             f"{'n/a' if rf.get('frac_dram') is None else format(rf['frac_dram'], '.2f')} of peak.  Parity in the same run: "
             + ", ".join(f"{p['config']}: {'bit-exact' if p['bit_exact'] else 'MISMATCH'}" for p in d.get("parity") or []) + ".")
+    if d.get("gpu"):
+        out += f"  Card: {d['gpu']['name']}, power limit {d['gpu']['power_limit']}, max SM clock {d['gpu']['sm_max_clock']}."
     if d.get("clocks"):
         out += f"  Clocks during the timed region: {d['clocks']['sm_mhz']} / {d['clocks']['sm_max_mhz']} MHz, reasons {d['clocks']['reasons']}."
     return out

@@ -26,7 +26,7 @@ def main():
         m = re.match(r"\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_.]*)", line)
         if m and cur is not None:
             cur[m.group(1)] += 1
-    out = [f"# cuobjdump opcode summary of libjosefine_b200.so (sm_100a), {tag} (tools/sass_summary.py)",
+    out = [f"# cuobjdump opcode summary of libjosefine_b200.so (sm_90a), {tag} (tools/sass_summary.py)",
            "# 128-bit global accesses = LDG.E.128 / STG.E.128 (state planes, mailbox units, Instruction FIFO);",
            "# LDS/STS.128 = shared-memory mailboxes and block-table cache; BAR.SYNC = the per-tick barrier;",
            "# POPC = quorum tally, FLO/BREV = __ffs over delivery masks; ATOMG.ADD = the split-launch task ticket,",
@@ -37,6 +37,7 @@ def main():
         out += [f"{short}  {sum(c.values())} SASS instructions", f"  memory : {fmt(MEM)}", f"  sync/vote/bit : {fmt(SYNC)}",
                 f"  tensor/TMA : {fmt(TENSOR) if fmt(TENSOR) != '-' else 'none (by design: integer state machine, no dense contraction)'}", ""]
     path = os.path.join(ROOT, "profiles", f"{tag}_sass_summary.txt")
+    os.makedirs(os.path.dirname(path), exist_ok=True)
     with open(path, "w") as f:
         f.write("\n".join(out))
     print(path, len(funcs), "functions")
