@@ -27,6 +27,9 @@
  *   jr_fsm_expand      <- Instruction::{Apply,Notify}         src/raft/fsm.rs:19-29, one per record element
  *   jr_node_restart    <- RaftHandle::new over an existing data directory: Chain::new reopening a
  *                         persisted chain                     src/raft/chain.rs:117-137
+ *   jr_node_restart_many <- RaftHandle::new over many existing data directories (one per (group, node)) in one call
+ *   jr_chain_export_many <- the sled trees of many nodes: the block records and the "commit" key
+ *                         Chain::new / append / extend / commit writing sled  src/raft/chain.rs:119-123,160-205
  *   jr_query_many / jr_chain_read_many <- the same pub fields, for many replicas in one call
  *   jr_engine_save / jr_engine_restore <- checkpoint of the whole engine (no reference API: sled persistence of
  *                         every node at once, chain.rs:119-123,198, plus the volatile State the reference loses)
@@ -507,6 +510,39 @@ jr_status jr_set_auto_truncate(jr_engine* e, int enabled, uint32_t margin);
  */
 jr_status jr_node_restart(jr_engine* e, uint32_t group, uint32_t node, uint64_t now_ms, const jr_block* blocks,
                           size_t n_blocks, uint64_t commit, int commit_key);
+
+/* One replica's persisted sled tree (chain.rs:99-104): its block records + the "commit" key.  32 bytes. */
+typedef struct jr_persisted_chain {
+  uint32_t group;
+  uint32_t node;         /* 1..R */
+  uint64_t commit;       /* value of the "commit" key (chain.rs:198) */
+  uint64_t first_block;  /* this replica's blocks are blocks[first_block .. first_block + n_blocks) */
+  uint32_t n_blocks;     /* restart only: JR_RESTART_IN_PLACE = reopen the replica's own table */
+  uint32_t commit_key;   /* the key exists (D6) */
+} jr_persisted_chain;
+#define JR_RESTART_IN_PLACE 0xFFFFFFFFu
+
+/*
+ * Bulk export: for target i = (groups[i], nodes[i]) every block present in the replica's window
+ * [floor, floor + chain_capacity), ascending id, as {id, next, token}, plus its commit and commit-key bit.
+ * out[i] describes target i (request order; targets may repeat); first_block is the running sum of the counts.
+ * *n_blocks = blocks needed.  blocks == NULL or cap_blocks < *n_blocks: `out` is filled, JR_E_CAPACITY.
+ * Faulted and silenced replicas are exported too (their sled tree still exists).  Synchronous.
+ */
+jr_status jr_chain_export_many(jr_engine* e, const uint32_t* groups, const uint32_t* nodes, size_t n,
+                               jr_persisted_chain* out, jr_block* blocks, size_t cap_blocks, size_t* n_blocks);
+/*
+ * Bulk restart: bit for bit n jr_node_restart(e, chains[i].group, chains[i].node, now_ms,
+ * blocks + chains[i].first_block, chains[i].n_blocks, chains[i].commit, chains[i].commit_key) calls in array order.
+ * n_blocks == JR_RESTART_IN_PLACE reopens the replica's own table (a crash that lost nothing: the reference writes
+ * every block and commit through to sled) -- the same as exporting it and restarting from the export; first_block,
+ * commit and commit_key are then ignored.  All or nothing: JR_E_INVAL, engine untouched, unless every group / node
+ * is in range, no (group, node) appears twice, every slice lies inside `blocks` and holds at most chain_capacity
+ * blocks with strictly ascending ids inside [floor, floor + chain_capacity) and next < 2^32-1, and every
+ * commit < 2^32-1.  Synchronous.
+ */
+jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted_chain* chains, size_t n,
+                               const jr_block* blocks, size_t n_blocks);
 /* Checkpoint: everything the engine holds (state planes, block tables, mailboxes, FIFOs, routing, counters).
  * jr_engine_save_size -> bytes needed; restore needs an engine created with the same jr_config. */
 jr_status jr_engine_save_size(jr_engine* e, size_t* bytes);

@@ -181,6 +181,47 @@ extern "C" {
     fn jr_fsm_records_async(e: *mut c_void) -> c_int;
     #[allow(dead_code)]
     fn jr_fsm_records_wait(e: *mut c_void, records: *mut *const c_void, batch: *mut c_void) -> c_int;
+    #[allow(dead_code)]
+    fn jr_chain_export_many(e: *mut c_void, groups: *const u32, nodes: *const u32, n: usize, out: *mut JrPersistedChain,
+                            blocks: *mut JrBlock, cap_blocks: usize, n_blocks: *mut usize) -> c_int;
+    #[allow(dead_code)]
+    fn jr_node_restart_many(e: *mut c_void, now_ms: u64, chains: *const JrPersistedChain, n: usize, blocks: *const JrBlock,
+                            n_blocks: usize) -> c_int;
+}
+
+/// One replica's persisted sled tree (chain.rs:99-104): blocks[first_block .. first_block + n_blocks] + the commit key.
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct JrPersistedChain {
+    pub group: u32,
+    pub node: u32,
+    pub commit: u64,
+    pub first_block: u64,
+    pub n_blocks: u32, // JR_RESTART_IN_PLACE: reopen the replica's own table
+    pub commit_key: u32,
+}
+#[allow(dead_code)]
+const JR_RESTART_IN_PLACE: u32 = 0xFFFF_FFFF;
+
+/// Sketch: what `Server::run` of a broker hosting node `id` of `n_groups` groups would do at start-up instead of one
+/// `RaftHandle::new` per group -- reopen every hosted group from the trees it kept, in ONE call.  `trees[g]` is
+/// (commit, commit key present, blocks) as read back from the host's store (`jr_chain_export_many` wrote them).
+#[allow(dead_code)]
+unsafe fn restart_hosted_groups(engine: *mut c_void, id: u32, now_ms: u64, trees: &[(u64, bool, Vec<JrBlock>)]) -> c_int {
+    let mut chains = Vec::with_capacity(trees.len());
+    let mut blocks = Vec::new();
+    for (g, (commit, key, bl)) in trees.iter().enumerate() {
+        chains.push(JrPersistedChain {
+            group: g as u32,
+            node: id,
+            commit: *commit,
+            first_block: blocks.len() as u64,
+            n_blocks: bl.len() as u32,
+            commit_key: *key as u32,
+        });
+        blocks.extend_from_slice(bl);
+    }
+    jr_node_restart_many(engine, now_ms, chains.as_ptr(), chains.len(), blocks.as_ptr(), blocks.len())
 }
 
 // Command discriminants, in the order of `enum Command` (src/raft/mod.rs:160-227)

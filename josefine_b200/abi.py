@@ -166,11 +166,20 @@ class LeaderEntry(C.Structure):
     _fields_ = [("term", C.c_uint64), ("leader_id", C.c_uint32), ("commit", C.c_uint32)]
 
 
+RESTART_IN_PLACE = 0xFFFFFFFF
+
+
+class PersistedChain(C.Structure):
+    """jr_persisted_chain: one replica's sled tree -- blocks[first_block : first_block + n_blocks] and the commit key."""
+    _fields_ = [("group", C.c_uint32), ("node", C.c_uint32), ("commit", C.c_uint64), ("first_block", C.c_uint64),
+                ("n_blocks", C.c_uint32), ("commit_key", C.c_uint32)]
+
+
 # sizes the header implies (checked in tests/test_abi.py against offsetof-free arithmetic)
 EXPECTED_SIZES = {
     "Config": 72, "Block": 24, "Msg": 64 + 24 * MAX_AE_BLOCKS, "FsmInstr": 16 + 24,
     "Proposal": 16, "TokenRun": 16, "LeaderEntry": 16, "FsmRecord": 32, "FsmBatch": 24 + 4 * (MAX_REPLICAS + 1) + 4,
-    "ReplicaState": 160,
+    "ReplicaState": 160, "PersistedChain": 32,
 }
 
 # every symbol include/josefine_raft_abi.h declares
@@ -180,7 +189,7 @@ ENGINE_SYMBOLS = [
     "jr_chain_read", "jr_state_digest", "jr_stream_digest", "jr_fault_count", "jr_fold_count", "jr_compact",
     "jr_set_alive", "jr_kill_leaders", "jr_leader_table_device", "jr_leader_table", "jr_leader_table_async", "jr_leader_table_wait",
     "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
-    "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
+    "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
 ]
 
 

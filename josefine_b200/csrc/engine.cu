@@ -511,20 +511,85 @@ __global__ void truncate_kernel(const Dev d, uint32_t margin, const uint8_t* ski
   d.tb[g] = floor;
 }
 
-// jr_node_restart: Chain::new over persisted blocks (chain.rs:117-137) + Raft::<Follower>::new (follower.rs:68-95)
-// for one replica.  Single thread; `blocks` is device memory.
-__global__ void node_restart_kernel(const Dev d, uint32_t g, uint32_t r, uint64_t now, const jr_block* blocks, uint32_t n,
-                                    uint32_t commit, uint32_t ckey) {
+// ---- bulk chain export / node restart ---------------------------------------------------------
+// One thread per requested replica, looping over table rows: the tables are [row][replica][group], so a warp of
+// group-consecutive requests (node k of every group -- the usual restart) touches each row coalesced.
+
+// The part of replica i's window that can hold blocks: ids [floor, floor + span).  Only inserts raise the largest key
+// (truncation zeroes it once the floor passes it), so nothing above it is present.
+__device__ __forceinline__ uint32_t window_span(const Dev& d, size_t i, uint32_t floor) {
+  const uint32_t mk = d.mk[i];
+  return mk < floor ? 0u : min(mk - floor + 1u, d.cap);
+}
+
+// jr_chain_export_many, pass 1: target k = {group, node - 1}; its descriptor with the number of blocks present
+// (first_block is the host's exclusive scan of those counts).
+__global__ void export_count_kernel(const Dev d, const uint2* targets, uint32_t n, jr_persisted_chain* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint2 t = targets[k];
+  const size_t plane = (size_t)d.R * d.Gp;
+  const size_t i = (size_t)t.y * d.Gp + t.x;
+  const uint32_t floor = d.tb[t.x], span = window_span(d, i, floor);
+  uint32_t cnt = 0;
+  for (uint32_t b = 0; b < span; ++b) cnt += d.cnext[(size_t)((floor + b) & d.capm) * plane + i] != ABSENT ? 1u : 0u;
+  const uint4 c = d.p2[i];
+  jr_persisted_chain o;
+  o.group = t.x;
+  o.node = t.y + 1;
+  o.commit = c.y;
+  o.first_block = 0;
+  o.n_blocks = cnt;
+  o.commit_key = (c.w >> 28) & 1u;
+  out[k] = o;
+}
+
+// jr_chain_export_many, pass 2: target k's blocks, ascending id, to out[first_block ..].
+__global__ void export_pack_kernel(const Dev d, const jr_persisted_chain* desc, uint32_t n, jr_block* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const jr_persisted_chain c = desc[k];
+  const size_t plane = (size_t)d.R * d.Gp;
+  const size_t i = (size_t)(c.node - 1) * d.Gp + c.group;
+  const uint32_t floor = d.tb[c.group], span = window_span(d, i, floor);
+  jr_block* o = out + c.first_block;
+  for (uint32_t b = 0, j = 0; b < span && j < c.n_blocks; ++b) {
+    const size_t row = (size_t)((floor + b) & d.capm) * plane + i;
+    const uint32_t nx = d.cnext[row];
+    if (nx != ABSENT) o[j++] = jr_block{(uint64_t)floor + b, nx, d.ctok[row]};
+  }
+}
+
+// jr_node_restart_many: Chain::new over a persisted tree (chain.rs:117-137) + Raft::<Follower>::new (follower.rs:68-95),
+// request k = reqs[k].  Host-validated: distinct replicas; ids strictly ascending inside [floor, floor + cap).  From host
+// data the window is emptied (an empty sled tree) and refilled; JR_RESTART_IN_PLACE keeps the rows and takes commit and
+// the commit key from the replica's own P2 -- the tree as the old incarnation left it.
+__global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persisted_chain* reqs, uint32_t n, const jr_block* blocks) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const jr_persisted_chain q = reqs[k];
+  const uint32_t g = q.group, r = q.node - 1;
   const size_t plane = (size_t)d.R * d.Gp;
   const size_t i = (size_t)r * d.Gp + g;
   const uint32_t floor = d.tb[g];
-  for (uint32_t b = 0; b < d.cap; ++b) d.cnext[(size_t)((floor + b) & d.capm) * plane + i] = ABSENT;  // an empty sled tree
-  uint32_t mk = 0;
-  for (uint32_t k = 0; k < n; ++k) {   // host-validated: floor <= id < floor + cap
-    const uint32_t bid = (uint32_t)blocks[k].id;
-    d.cnext[(size_t)(bid & d.capm) * plane + i] = (uint32_t)blocks[k].next;
-    d.ctok[(size_t)(bid & d.capm) * plane + i] = blocks[k].data;
-    mk = max(mk, bid);
+  uint32_t commit, ckey, mk = 0;
+  if (q.n_blocks == JR_RESTART_IN_PLACE) {
+    const uint4 c = d.p2[i];
+    commit = c.y;
+    ckey = (c.w >> 28) & 1u;
+    for (uint32_t b = window_span(d, i, floor); b-- > 0;)   // the largest key becomes exact, as an export would make it
+      if (d.cnext[(size_t)((floor + b) & d.capm) * plane + i] != ABSENT) { mk = floor + b; break; }
+  } else {
+    commit = (uint32_t)q.commit;
+    ckey = q.commit_key ? 1u : 0u;
+    for (uint32_t b = 0; b < d.cap; ++b) d.cnext[(size_t)((floor + b) & d.capm) * plane + i] = ABSENT;
+    const jr_block* bl = blocks + q.first_block;
+    for (uint32_t j = 0; j < q.n_blocks; ++j) {
+      const uint32_t bid = (uint32_t)bl[j].id;
+      d.cnext[(size_t)(bid & d.capm) * plane + i] = (uint32_t)bl[j].next;
+      d.ctok[(size_t)(bid & d.capm) * plane + i] = bl[j].data;
+      mk = bid;                        // ascending: the last one is the largest
+    }
   }
   uint32_t idgen = commit;             // IdGenerator::new(commit), chain.rs:126
   if (commit == 0) {                   // chain.init(), chain.rs:139-153: id_gen.next() == 0, block 0 -> 0 inserted
@@ -2172,26 +2237,138 @@ jr_status jr_set_auto_truncate(jr_engine* e, int enabled, uint32_t margin) {
   return JR_OK;
 }
 
+jr_status jr_chain_export_many(jr_engine* e, const uint32_t* groups, const uint32_t* nodes, size_t n,
+                               jr_persisted_chain* out, jr_block* blocks, size_t cap_blocks, size_t* n_blocks) {
+  if (!e || !n_blocks || (n && (!groups || !nodes || !out))) return JR_E_INVAL;
+  *n_blocks = 0;
+  if (n == 0) return JR_OK;
+  if (n > 0x7fffffffu) return JR_E_INVAL;
+  std::vector<uint2> targets(n);
+  for (size_t k = 0; k < n; ++k) {
+    if (groups[k] >= e->d.G || nodes[k] < 1 || nodes[k] > e->d.R) {
+      set_err("target %zu: group or node out of range", k);
+      return JR_E_INVAL;
+    }
+    targets[k] = make_uint2(groups[k], nodes[k] - 1);
+  }
+  CK(cudaSetDevice(e->cfg.device));
+  // pass 1: descriptors with counts -> host.  The scan over the counts runs here: the descriptors have to reach the
+  // caller anyway, and the call synchronises, so a device scan would save no round trip.
+  const size_t o_desc = (n * sizeof(uint2) + 15) / 16 * 16;
+  jr_status st = many_reserve(e, o_desc + n * sizeof(jr_persisted_chain));
+  if (st != JR_OK) return st;
+  char* base = (char*)e->many_buf;
+  CK(cudaMemcpyAsync(base, targets.data(), n * sizeof(uint2), cudaMemcpyHostToDevice, e->stream));
+  JR_LAUNCH(export_count_kernel, (unsigned)((n + 127) / 128), 128, e->stream, e->d, (const uint2*)base, (uint32_t)n,
+            (jr_persisted_chain*)(base + o_desc));
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out, base + o_desc, n * sizeof(jr_persisted_chain), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));   // (also covers `targets`, which lives on this stack)
+  uint64_t total = 0;
+  for (size_t k = 0; k < n; ++k) {
+    out[k].first_block = total;
+    total += out[k].n_blocks;
+  }
+  *n_blocks = (size_t)total;
+  if (!blocks || cap_blocks < total) return JR_E_CAPACITY;
+  if (total == 0) return JR_OK;
+  // pass 2: the blocks, packed in request order into a staging buffer, then one copy out
+  const size_t o_blk = (n * sizeof(jr_persisted_chain) + 15) / 16 * 16;
+  if ((st = many_reserve(e, o_blk + total * sizeof(jr_block))) != JR_OK) return st;
+  base = (char*)e->many_buf;
+  CK(cudaMemcpyAsync(base, out, n * sizeof(jr_persisted_chain), cudaMemcpyHostToDevice, e->stream));
+  JR_LAUNCH(export_pack_kernel, (unsigned)((n + 127) / 128), 128, e->stream, e->d, (const jr_persisted_chain*)base,
+            (uint32_t)n, (jr_block*)(base + o_blk));
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(blocks, base + o_blk, total * sizeof(jr_block), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
+}
+
+jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted_chain* chains, size_t n,
+                               const jr_block* blocks, size_t n_blocks) {
+  if (!e || (n && !chains) || (n_blocks && !blocks)) return JR_E_INVAL;
+  if (n == 0) return JR_OK;
+  if (n > 0x7fffffffu) return JR_E_INVAL;
+  const Dev& d = e->d;
+  // everything is checked before the first device write: on JR_E_INVAL the engine is untouched
+  uint32_t g_lo = 0xffffffffu, g_hi = 0;   // the groups the call names lie in [g_lo, g_hi]
+  for (size_t k = 0; k < n; ++k) {
+    if (chains[k].group >= d.G || chains[k].node < 1 || chains[k].node > d.R) {
+      set_err("chains[%zu]: group or node out of range", k);
+      return JR_E_INVAL;
+    }
+    g_lo = std::min(g_lo, chains[k].group);
+    g_hi = std::max(g_hi, chains[k].group);
+  }
+  const size_t span = (size_t)g_hi - g_lo + 1;
+  std::vector<uint8_t> seen(span * d.R, 0);
+  bool host_blocks = false;
+  for (size_t k = 0; k < n; ++k) {
+    const jr_persisted_chain& c = chains[k];
+    uint8_t& s = seen[(size_t)(c.node - 1) * span + (c.group - g_lo)];
+    if (s) {
+      set_err("chains[%zu]: replica (%u, %u) appears twice", k, c.group, c.node);
+      return JR_E_INVAL;
+    }
+    s = 1;
+    if (c.n_blocks == JR_RESTART_IN_PLACE) continue;
+    if (c.n_blocks > d.cap || c.first_block > n_blocks || n_blocks - c.first_block < c.n_blocks || c.commit >= 0xffffffffull) {
+      set_err("chains[%zu]: slice outside blocks[0, %zu), more than chain_capacity blocks, or commit >= 2^32-1", k, n_blocks);
+      return JR_E_INVAL;
+    }
+    host_blocks |= c.n_blocks > 0;
+  }
+  CK(cudaSetDevice(e->cfg.device));
+  if (host_blocks) {
+    std::vector<uint32_t> floor(span);   // the groups' floors: one copy of the TB plane's [g_lo, g_hi]
+    CK(cudaMemcpyAsync(floor.data(), d.tb + g_lo, span * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    for (size_t k = 0; k < n; ++k) {
+      const jr_persisted_chain& c = chains[k];
+      if (c.n_blocks == JR_RESTART_IN_PLACE) continue;
+      const uint64_t lo = floor[c.group - g_lo];
+      for (uint32_t j = 0; j < c.n_blocks; ++j) {
+        const jr_block& b = blocks[c.first_block + j];
+        if (b.id < lo || b.id - lo >= d.cap || b.next >= 0xffffffffull || (j && b.id <= blocks[c.first_block + j - 1].id)) {
+          set_err("chains[%zu] block %u: id not ascending or outside [floor, floor + chain_capacity), or next >= 2^32-1 (D4, D7)", k, j);
+          return JR_E_INVAL;
+        }
+      }
+    }
+  }
+  const size_t o_blk = (n * sizeof(jr_persisted_chain) + 15) / 16 * 16;
+  jr_status st = many_reserve(e, o_blk + n_blocks * sizeof(jr_block));
+  if (st != JR_OK) return st;
+  char* base = (char*)e->many_buf;
+  CK(cudaMemcpyAsync(base, chains, n * sizeof(jr_persisted_chain), cudaMemcpyHostToDevice, e->stream));
+  if (n_blocks) CK(cudaMemcpyAsync(base + o_blk, blocks, n_blocks * sizeof(jr_block), cudaMemcpyHostToDevice, e->stream));
+  JR_LAUNCH(node_restart_kernel, (unsigned)((n + 127) / 128), 128, e->stream, d, now_ms, (const jr_persisted_chain*)base,
+            (uint32_t)n, (const jr_block*)(base + o_blk));
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
+}
+
+// One replica: a one-element jr_node_restart_many.  `blocks` may come in any order and repeat an id; the table holds
+// the last copy of each id, so they are sorted stably and all but the last copy dropped first.
 jr_status jr_node_restart(jr_engine* e, uint32_t group, uint32_t node, uint64_t now_ms, const jr_block* blocks,
                           size_t n_blocks, uint64_t commit, int commit_key) {
   if (!e || group >= e->d.G || node < 1 || node > e->d.R || (n_blocks && !blocks)) return JR_E_INVAL;
   if (n_blocks > e->d.cap || commit >= 0xffffffffull) return JR_E_INVAL;
-  CK(cudaSetDevice(e->cfg.device));
-  jr_replica_state st0;
-  jr_status st = jr_query(e, group, node, &st0);   // (synchronises; also tells the group's floor)
-  if (st != JR_OK) return st;
-  for (size_t k = 0; k < n_blocks; ++k)
-    if (blocks[k].id < st0.chain_floor || blocks[k].id - st0.chain_floor >= e->d.cap || blocks[k].next >= 0xffffffffull) {
-      set_err("blocks[%zu]: id outside [floor, floor + chain_capacity) or next >= 2^32-1 (D4, D7)", k);
-      return JR_E_INVAL;
-    }
-  if ((st = many_reserve(e, std::max<size_t>(n_blocks, 1) * sizeof(jr_block))) != JR_OK) return st;
-  if (n_blocks) CK(cudaMemcpyAsync(e->many_buf, blocks, n_blocks * sizeof(jr_block), cudaMemcpyHostToDevice, e->stream));
-  JR_LAUNCH(node_restart_kernel, 1, 1, e->stream, e->d, group, node - 1, now_ms, (const jr_block*)e->many_buf,
-            (uint32_t)n_blocks, (uint32_t)commit, commit_key ? 1u : 0u);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(e->stream));
-  return JR_OK;
+  std::vector<jr_block> v(blocks, blocks + n_blocks);
+  std::stable_sort(v.begin(), v.end(), [](const jr_block& a, const jr_block& b) { return a.id < b.id; });
+  size_t m = 0;
+  for (size_t k = 0; k < v.size(); ++k)
+    if (k + 1 == v.size() || v[k + 1].id != v[k].id) v[m++] = v[k];
+  jr_persisted_chain c;
+  c.group = group;
+  c.node = node;
+  c.commit = commit;
+  c.first_block = 0;
+  c.n_blocks = (uint32_t)m;
+  c.commit_key = commit_key ? 1u : 0u;
+  return jr_node_restart_many(e, now_ms, &c, 1, v.data(), m);
 }
 
 // ---- checkpoint -----------------------------------------------------------------------------------

@@ -12,8 +12,8 @@ bincode 1.3 (default options: fixed-width little-endian integers, u64 lengths) o
   Vec<u8>                                ->  u64 len + bytes
 so a Block record is  08 00.. | id_be8 | 08 00.. | next_be8 | len_le8 | data.
 
-What this module does: turn one replica's device-resident block table (`jr_chain_read`) into that
-ordered (key, value) record list and back.  What it does NOT do: write sled's own page/log file
+What this module does: turn replicas' device-resident block tables (`jr_chain_export_many`) into that
+ordered (key, value) record list and back (`jr_node_restart_many`).  What it does NOT do: write sled's own page/log file
 format (sled 0.34.7 is a third-party dependency that is not vendored in the reference, and
 its file layout is not something to restate from memory) -- a josefine-side loader is one
 `db.insert(k, v)` loop over these records.  **Parity unpinned**: no Rust toolchain here, the byte
@@ -56,25 +56,32 @@ def decode_block(value: bytes) -> Tuple[int, int, bytes]:
     return int.from_bytes(idb, "big"), int.from_bytes(nxb, "big"), data
 
 
+def _records(commit: int, commit_key: bool, blocks, payloads: Optional[Dict[int, bytes]]) -> List[Tuple[bytes, bytes]]:
+    recs = []
+    for bid, nxt, tok in blocks:
+        data = payloads[tok] if payloads is not None and tok in payloads else (struct.pack("<Q", tok) if tok else b"")
+        recs.append((block_key(bid), encode_block(bid, nxt, data)))
+    if commit_key:                          # the key only exists once Chain::commit has run (chain.rs:198)
+        recs.append((COMMIT_KEY, block_key(commit)))
+    recs.sort(key=lambda kv: kv[0])
+    return recs
+
+
+def export_many(api, targets: Iterable[Tuple[int, int]],
+                payloads: Optional[Dict[int, bytes]] = None) -> Dict[Tuple[int, int], List[Tuple[bytes, bytes]]]:
+    """`chain_records` of many replicas through one `chain_export_many` call: {(group, node): records}."""
+    targets = list(targets)
+    return {(g, n): _records(commit, ck, blocks, payloads)
+            for (g, n), (commit, ck, blocks) in zip(targets, api.chain_export_many(targets))}
+
+
 def chain_records(api, group: int, node: int, payloads: Optional[Dict[int, bytes]] = None) -> List[Tuple[bytes, bytes]]:
     """Every record josefine's sled tree would hold for replica (group, node), in sled's key order.
 
     `payloads` maps the engine's 64-bit block tokens to the payload bytes the host kept (deviation D5);
     a token without an entry is written as its own 8 little-endian bytes so the record stays reversible.
     """
-    st = api.query(group, node)
-    blocks = api.chain_read(group, node, 0, int(st.max_key) + 1)
-    recs = []
-    for b in blocks:
-        if b is None:
-            continue
-        bid, nxt, tok = b
-        data = payloads[tok] if payloads is not None and tok in payloads else (struct.pack("<Q", tok) if tok else b"")
-        recs.append((block_key(bid), encode_block(bid, nxt, data)))
-    if st.commit > 0:                       # the key only exists once Chain::commit has run (chain.rs:198)
-        recs.append((COMMIT_KEY, block_key(st.commit)))
-    recs.sort(key=lambda kv: kv[0])
-    return recs
+    return export_many(api, [(group, node)], payloads)[(group, node)]
 
 
 def reopen(records: Iterable[Tuple[bytes, bytes]]) -> dict:
@@ -122,3 +129,14 @@ def restart_from_records(api, group: int, node: int, now_ms: int, records, token
     records = list(records)
     blocks, commit, commit_key = import_records(records, tokens)
     api.node_restart(group, node, now_ms, blocks, commit, commit_key)
+
+
+def restart_many_from_records(api, now_ms: int, trees: Dict[Tuple[int, int], Iterable[Tuple[bytes, bytes]]],
+                              tokens: Optional[Dict[bytes, int]] = None):
+    """`RaftHandle::new` over many data directories at once: trees = {(group, node): records}, one
+    `node_restart_many` call."""
+    chains = []
+    for (g, n), records in trees.items():
+        blocks, commit, commit_key = import_records(list(records), tokens)
+        chains.append((g, n, blocks, commit, commit_key))
+    api.node_restart_many(now_ms, chains)

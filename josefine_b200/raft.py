@@ -405,6 +405,69 @@ class RaftApi:
         self._check(self._fn("node_restart")(self._h, C.c_uint32(group), C.c_uint32(node), C.c_uint64(now_ms), arr,
                                              C.c_size_t(len(blocks)), C.c_uint64(commit), C.c_int(int(ck))), "node_restart")
 
+    def chain_export_many(self, targets: Sequence[Tuple[int, int]]) -> List[Tuple[int, bool, List[Tuple[int, int, int]]]]:
+        """jr_chain_export_many: each (group, node)'s persisted sled tree as (commit, commit_key, [(id, next, token)]),
+        every block present in the replica's window, ascending id.  Without the batched call (the oracle): query +
+        chain_read per target, and the commit key is taken to exist once something was committed."""
+        targets = list(targets)
+        n = len(targets)
+        if not hasattr(self._lib, self._p + "chain_export_many"):
+            out = []
+            for g, nd in targets:
+                st = self.query(g, nd)
+                lo = int(st.chain_floor)
+                hi = min(int(st.max_key), lo + self.cfg.chain_capacity - 1)
+                blocks = [b for b in self.chain_read(g, nd, lo, hi - lo + 1) if b is not None] if hi >= lo else []
+                out.append((int(st.commit), st.commit > 0, blocks))
+            return out
+        gs = (C.c_uint32 * max(n, 1))(*[t[0] for t in targets])
+        ns = (C.c_uint32 * max(n, 1))(*[t[1] for t in targets])
+        desc = (abi.PersistedChain * max(n, 1))()
+        need = C.c_size_t(0)
+        fn = self._fn("chain_export_many")
+        st = fn(self._h, gs, ns, C.c_size_t(n), desc, None, C.c_size_t(0), C.byref(need))
+        if st != abi.E_CAPACITY:
+            self._check(st, "chain_export_many")
+        blk = (abi.Block * max(need.value, 1))()
+        if need.value:
+            self._check(fn(self._h, gs, ns, C.c_size_t(n), desc, blk, need, C.byref(need)), "chain_export_many")
+        out = []
+        for i in range(n):
+            d = desc[i]
+            out.append((d.commit, bool(d.commit_key),
+                        [(blk[j].id, blk[j].next, blk[j].data) for j in range(d.first_block, d.first_block + d.n_blocks)]))
+        return out
+
+    def node_restart_many(self, now_ms: int,
+                          chains: Sequence[Tuple[int, int, Optional[Sequence[Tuple[int, int, int]]], int, Optional[bool]]]):
+        """jr_node_restart_many: chains = [(group, node, blocks, commit, commit_key)]; blocks None = in place (the replica
+        reopens its own table and commit; commit and commit_key are ignored), commit_key None = (commit > 0).  Without
+        the batched call (the oracle): one node_restart per entry, in order, in place = from its own export."""
+        chains = list(chains)
+        if not hasattr(self._lib, self._p + "node_restart_many"):
+            for g, nd, blocks, commit, ck in chains:
+                if blocks is None:
+                    commit, ck, blocks = self.chain_export_many([(g, nd)])[0]
+                self.node_restart(g, nd, now_ms, blocks, commit, ck)
+            return
+        n = len(chains)
+        desc = (abi.PersistedChain * max(n, 1))()
+        flat: List[Tuple[int, int, int]] = []
+        for i, (g, nd, blocks, commit, ck) in enumerate(chains):
+            d = desc[i]
+            d.group, d.node = g, nd
+            if blocks is None:
+                d.n_blocks = abi.RESTART_IN_PLACE
+                continue
+            d.commit, d.first_block, d.n_blocks = commit, len(flat), len(blocks)
+            d.commit_key = int((commit > 0) if ck is None else bool(ck))
+            flat.extend(blocks)
+        arr = (abi.Block * max(len(flat), 1))()
+        for i, (bid, nxt, data) in enumerate(flat):
+            arr[i].id, arr[i].next, arr[i].data = bid, nxt, data
+        self._check(self._fn("node_restart_many")(self._h, C.c_uint64(now_ms), desc, C.c_size_t(n), arr,
+                                                  C.c_size_t(len(flat))), "node_restart_many")
+
     def save(self) -> bytes:
         """jr_engine_save: checkpoint of everything the engine holds."""
         n = C.c_size_t(0)
@@ -492,6 +555,9 @@ def _bind(lib: C.CDLL, p: str):
                             C.c_size_t, C.POINTER(abi.Block), C.POINTER(C.c_uint8)],
         "truncate": [vp, C.c_uint32],
         "node_restart": [vp, C.c_uint32, C.c_uint32, C.c_uint64, C.POINTER(abi.Block), C.c_size_t, C.c_uint64, C.c_int],
+        "chain_export_many": [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(abi.PersistedChain),
+                              C.POINTER(abi.Block), C.c_size_t, C.POINTER(C.c_size_t)],
+        "node_restart_many": [vp, C.c_uint64, C.POINTER(abi.PersistedChain), C.c_size_t, C.POINTER(abi.Block), C.c_size_t],
         "engine_save_size": [vp, C.POINTER(C.c_size_t)],
         "engine_save": [vp, C.c_void_p, C.c_size_t],
         "engine_restore": [vp, C.c_void_p, C.c_size_t],

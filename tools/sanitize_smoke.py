@@ -52,6 +52,10 @@ for R, G in ((3, 70), (5, 96)):
     e.chain_read_many([(g, 1, int(st[g].chain_floor), 8) for g in range(0, G, 9)])
     blocks = [b for b in e.chain_read(0, 2, int(st[0].chain_floor), 40) if b is not None]
     e.node_restart(0, 2, now, blocks, int(e.query(0, 2).commit))
+    # bulk export + restart: node 2 of every group from its export, node 3 of every other group in place
+    exp = e.chain_export_many([(g, 2) for g in range(G)])
+    e.node_restart_many(now, [(g, 2, bl, c, ck) for g, (c, ck, bl) in enumerate(exp)] +
+                        [(g, 3, None, 0, None) for g in range(0, G, 2)])
     e.run(now, 100, 6, 1)
     print(R, "folded per launch", folded, e.state_digest(), e.fault_count())
 # the one-lane fold (A/B and fallback path) once as well
