@@ -45,6 +45,20 @@ struct SymMail {
   uint32_t mk;                            // the leader's largest block id when it sent this (sym2_kernel: which cache slots it may be rewriting)
   uint32_t hbr, hbr_commit, hbr_has;      // followers -> leader
   uint32_t ar, ar_head;
+  // read / write ae_id[k] for a k known only at run time through static indices: an array indexed dynamically lives in
+  // local memory (with it, the mail of every tick did)
+  __device__ __forceinline__ uint32_t id(uint32_t k) const {
+    uint32_t v = ae_id[0];
+#pragma unroll
+    for (uint32_t j = 1; j < JR_MAX_AE_BLOCKS; ++j)
+      if (k == j) v = ae_id[j];
+    return v;
+  }
+  __device__ __forceinline__ void set_id(uint32_t k, uint32_t v) {
+#pragma unroll
+    for (uint32_t j = 0; j < JR_MAX_AE_BLOCKS; ++j)
+      if (k == j) ae_id[j] = v;
+  }
 };
 
 // Block-table rows the fold has touched recently, per lane, in SHARED memory: two direct-mapped caches (the leader's
@@ -77,6 +91,23 @@ constexpr uint32_t SYM_SMEM_UNITS = 2 * SYM_ROWS + SYM_ENC_L + SYM_ENC_F;   // u
 constexpr uint32_t SYM2_GROUPS = 64;                                        // groups per CTA: 128 threads
 constexpr uint32_t SYM2_UNITS = SYM_SMEM_UNITS + 2 * 2 + 2 * 1;            // uint4 per group
 constexpr uint32_t SYM2_ABORT = 1u << 8, SYM2_IDS = 1u << 9, SYM2_MODE = 1u << 10;
+// Phase profile of sym2_kernel (JR_PROFILE builds only, tools/sym2_profile.py): the slots of the per-(role, slot) cycle
+// counters.  The leader lane counts under JR_ROLE_LEADER, the follower lane under JR_ROLE_FOLLOWER; each cycle of a tick
+// goes to exactly one slot.
+enum : uint32_t {
+  SP_MAIL_IN = 0,      // read the other lane's mail (leader: and this tick's proposal)
+  SP_AR = 1,           // leader: AppendResponse, the leader_commit loop
+  SP_CLIENT = 2,       // leader: client_request -- row stores, cache put, the commit check after it
+  SP_ENC_NOTIFY = 3,   // leader: NOTIFY encoder pushes
+  SP_ENC_APPLY = 4,    // APPLY encoder pushes (leader: what a commit applies; followers: the apply range)
+  SP_MAIL_OUT = 5,     // leader: the heartbeat decision; both: the mail write
+  SP_BARRIER = 6,      // waiting at the per-tick barrier
+  SP_HB = 7,           // followers: Heartbeat and its apply range
+  SP_SCAN = 8,         // followers: the replicate() scan over the leader's rows (fetch_sent)
+  SP_EXTEND = 9,       // followers: follower_extend, the R-1 row stores
+  SP_ENTER = 10, SP_FILL = 11, SP_LEAVE = 12, SP_TRUNC = 13,   // once per launch: sym_enter (with its barriers), cache fill +
+                                                               // encoder init, sym_leave_*, the fused truncation
+};
 
 template <int R, bool SPLIT = false>
 struct SymGroup {
@@ -96,11 +127,32 @@ struct SymGroup {
   uint4* rows;                             // this lane's column of the CTA's row caches (see above)
   uint4* enc;                              // this lane's column of the encoder states (see above)
   uint32_t lcnt, fcnt;                     // raw Instructions emitted: leader / each follower
+  uint32_t lwend, fwend;                   // lcnt / fcnt at which the open pattern window is full (wseq - seq0 + FS_PATTERN_BITS)
   uint32_t n_app;                          // most blocks the leader can append in one tick (dense + synthetic proposals)
   bool abort;
   bool share;                              // the followers' Instruction FIFOs are all empty: their records can be shared
+#ifdef JR_PROFILE
+  long long pt;                            // clock64() at the last phase boundary
+  uint32_t prole, pslot;                   // profile role of this lane, phase its cycles go to now
+  // close the current phase (lane 0 of the warp adds the cycles since the last boundary to it), open `slot`; returns the
+  // phase it closed, so a nested phase can hand the time back to its caller's
+  __device__ __forceinline__ uint32_t phase(uint32_t slot) {
+    const uint32_t o = pslot;
+    if constexpr (SPLIT) {   // (sym_kernel is not profiled: its shared memory has no room for the counters)
+      JR_PROF_ADD(prole, o, pt);
+      pslot = slot;
+    }
+    return o;
+  }
+#else
+  __device__ __forceinline__ uint32_t phase(uint32_t) const { return 0; }
+#endif
 
-  __device__ __forceinline__ SymGroup(const Dev& dv, uint32_t g_) : d(dv), g(g_), plane((size_t)R * dv.Gp) {}
+  __device__ __forceinline__ SymGroup(const Dev& dv, uint32_t g_) : d(dv), g(g_), plane((size_t)R * dv.Gp) {
+#ifdef JR_PROFILE
+    pt = 0; prole = JR_ROLE_CANDIDATE; pslot = 0;
+#endif
+  }
   __device__ __forceinline__ size_t rg(uint32_t r) const { return (size_t)r * d.Gp + g; }
   __device__ __forceinline__ size_t row(uint32_t r, uint32_t bid) const { return (size_t)(bid & d.capm) * plane + rg(r); }
   __device__ __forceinline__ bool in_window(uint32_t bid) const { return bid - tbase < d.cap; }   // (sym_enter made sure ids stay below 2^31)
@@ -172,19 +224,51 @@ struct SymGroup {
   __device__ __forceinline__ FsmOut followers_out() const {   // one set of records for all followers: node mask in the APPLY records
     return FsmOut{d.fs + rg(F0), plane, d.F, g, F0, ((1u << R) - 1u) & ~(1u << L)};
   }
-  __device__ __forceinline__ void enc_init_leader(uint2 leader_fc) const {
+  __device__ __forceinline__ void enc_init_leader(uint2 leader_fc) {
     eq(0) = make_uint4(leader_fc.x, leader_fc.y, leader_fc.y, 0u);
 #pragma unroll
     for (uint32_t k = 1; k < SYM_ENC_L; ++k) eq(k) = make_uint4(0u, 0u, 0u, 0u);
+    lwend = FS_PATTERN_BITS;
   }
-  __device__ __forceinline__ void enc_init_followers() const {
+  __device__ __forceinline__ void enc_init_followers() {
 #pragma unroll
     for (uint32_t k = SYM_ENC_L; k < SYM_ENC_L + SYM_ENC_F; ++k) eq(k) = make_uint4(0u, 0u, 0u, 0u);
+    fwend = FS_PATTERN_BITS;
+  }
+  // The common case of fsm_enc_push, on a run parked in shared memory (q = {next_id, count, last}, qs = its stride): the
+  // run is open and (bid, nxa, tok) continues it.  Extends it in place and returns true; the caller has checked that
+  // this push does not fill the pattern window, so the push changes nothing else.  false: nothing was written.
+  template <bool NOTIFY>
+  __device__ __forceinline__ bool run_extend(uint4& q, uint2& qs, uint32_t bid, uint32_t nxa, uint64_t tok) const {
+    const uint4 r = q;
+    if (!r.y || bid != r.x || r.y >= FS_MAX_RUN || nxa != (NOTIFY ? FSR_CLIENT : bid - 1u)) return false;
+    const uint2 st = qs;
+    const uint64_t step = tok - ((uint64_t)r.z | ((uint64_t)r.w << 32));
+    if (r.y == 1u) {                                       // count 1: its own `next` / address must be regular too
+      if (st.x != (NOTIFY ? FSR_CLIENT : bid - 2u)) return false;
+      qs = make_uint2((uint32_t)step, (uint32_t)(step >> 32));
+    } else if (step != ((uint64_t)st.x | ((uint64_t)st.y << 32))) {
+      return false;
+    }
+    q = make_uint4(bid + 1u, r.y + 1u, (uint32_t)tok, (uint32_t)(tok >> 32));
+    return true;
   }
   template <bool NOTIFY>
   __device__ __forceinline__ void emit_leader(uint32_t bid, uint32_t nxa, uint64_t tok) {
     if (!(d.flags & JR_F_CAPTURE_FSM)) return;
     if (lcnt >= d.Fr) { abort = true; return; }          // step_kernel's raw FIFO would overflow (it drops and counts): its business
+    const uint32_t outer = phase(NOTIFY ? SP_ENC_NOTIFY : SP_ENC_APPLY);
+    if (lcnt + 1u != lwend &&
+        run_extend<NOTIFY>(eq(NOTIFY ? 4 : 2), reinterpret_cast<uint2*>(&eq(3))[NOTIFY ? 1 : 0], bid, nxa, tok)) {
+      if (NOTIFY) {                                        // the pattern bit seq - wseq: one word of e1 = {pb0, pb1} or e0.w = pb2
+        const uint32_t b = lcnt + FS_PATTERN_BITS - lwend;
+        uint32_t* w = b < 128u ? reinterpret_cast<uint32_t*>(&eq(1)) + (b >> 5) : &eq(0).w;
+        *w |= 1u << (b & 31u);
+      }
+      ++lcnt;
+      phase(outer);
+      return;
+    }
     FsmEnc e;
     const uint4 q0 = eq(0);
     e.nrec = q0.x; e.seq = q0.y + lcnt; e.wseq = q0.z; e.pb2 = q0.w;
@@ -205,6 +289,8 @@ struct SymGroup {
     eq(NOTIFY ? 4 : 2) = make_uint4(run.next_id, run.count, (uint32_t)run.last, (uint32_t)(run.last >> 32));
     uint2* st = reinterpret_cast<uint2*>(&eq(3)) + (NOTIFY ? 1 : 0);
     *st = make_uint2((uint32_t)run.stride, (uint32_t)(run.stride >> 32));
+    lwend = e.wseq - q0.y + FS_PATTERN_BITS;
+    phase(outer);
   }
   __device__ __forceinline__ uint2 leader_end() {          // close the leader's runs: its new {records, Instructions}
     FsmEnc e;
@@ -219,7 +305,11 @@ struct SymGroup {
   __device__ __forceinline__ void emit_followers(uint32_t bid, uint32_t next, uint64_t tok) {
     if (!(d.flags & JR_F_CAPTURE_FSM)) return;
     if (fcnt >= d.Fr) { abort = true; return; }
-    if (share) {                                           // encoded once, for all followers
+    const uint32_t outer = phase(SP_ENC_APPLY);
+    if (share && fcnt + 1u != fwend &&
+        run_extend<false>(eq(SYM_ENC_L + 1), *reinterpret_cast<uint2*>(&eq(SYM_ENC_L + 2)), bid, next, tok)) {
+      // extended in place (no Notify: no pattern bits)
+    } else if (share) {                                    // encoded once, for all followers
       FsmEnc e;
       const uint4 q0 = eq(SYM_ENC_L), q1 = eq(SYM_ENC_L + 1);
       const uint2 q2 = *reinterpret_cast<const uint2*>(&eq(SYM_ENC_L + 2));
@@ -230,6 +320,7 @@ struct SymGroup {
       if (e.nrec != q0.x || e.wseq != q0.z) eq(SYM_ENC_L) = make_uint4(e.nrec, q0.y, e.wseq, 0u);
       eq(SYM_ENC_L + 1) = make_uint4(e.ra.next_id, e.ra.count, (uint32_t)e.ra.last, (uint32_t)(e.ra.last >> 32));
       *reinterpret_cast<uint2*>(&eq(SYM_ENC_L + 2)) = make_uint2((uint32_t)e.ra.stride, (uint32_t)(e.ra.stride >> 32));
+      fwend = e.wseq - q0.y + FS_PATTERN_BITS;
     } else {                                               // followers with records pending: raw entries, fsm_flush at the end
       const uint4 e = make_uint4(bid, next, (uint32_t)tok, (uint32_t)(tok >> 32));
 #pragma unroll
@@ -237,6 +328,7 @@ struct SymGroup {
         if ((uint32_t)r != L) d.fr[(size_t)fcnt * plane + rg(r)] = e;
     }
     ++fcnt;
+    phase(outer);
   }
   __device__ __forceinline__ uint2 followers_end() {
     FsmEnc e;
@@ -305,6 +397,7 @@ struct SymGroup {
     // peer mail, ascending sender, FIFO per sender: every follower sent the same [HeartbeatResponse][AppendResponse]
     if (in.hbr && !in.hbr_has && in.hbr_commit > 0) { abort = true; return; }   // leader.rs:222-231 would replicate mid-drain
     if (in.ar) {
+      phase(SP_AR);
       const uint32_t old = ph_f, v = in.ar_head;
       const bool inc = old < v;                          // progress.rs:133-140, the same for every follower
       const uint32_t nw = inc ? v : old;
@@ -314,10 +407,12 @@ struct SymGroup {
       if (abort) return;
     }
     // client arm, server.rs:156-160: the dense proposal, then the synthetic ones
+    phase(SP_CLIENT);
     if (dense_tok) client_request(dense_tok);
     for (uint32_t i = 0; i < n_synth && !abort; ++i) client_request(synth_token(step_index, i, d.goff + g));
     if (abort) return;
     // Command::Tick, leader.rs:234-245
+    phase(SP_MAIL_OUT);
     const uint64_t el = now >= hbtime ? now - hbtime : 0;
     if (el > (uint64_t)d.hb) {
       out.hb = 1;
@@ -345,7 +440,7 @@ struct SymGroup {
         ++bid;
       }
       if (bid > mk) break;
-      if (pulled >= 1) out.ae_id[nb++] = bid;
+      if (pulled >= 1) out.set_id(nb++, bid);
       ++pulled;
       ++bid;
     }
@@ -354,7 +449,8 @@ struct SymGroup {
 
   // ---- follower (follower.rs), once for all R-1 of them ----------------------------------------------------------
   __device__ __forceinline__ void follower_heartbeat(const SymMail& in, SymMail& out) {   // follower.rs:178-217
-    ++n_hb;                                                // set_election_timeout: one RNG draw, timer restarted
+    phase(SP_HB);
+    ++n_hb;                                               // set_election_timeout: one RNG draw, timer restarted
     last_hb = now;
     const uint32_t c = in.hb_commit;
     const bool hasc = has_f(c);
@@ -374,6 +470,7 @@ struct SymGroup {
   }
   // one block of an AppendEntries, applied by every follower (follower.rs:156-173 -> chain.rs:180-190)
   __device__ __forceinline__ void follower_extend(uint32_t bid, uint32_t nx, uint64_t tk) {
+    const uint32_t outer = phase(SP_EXTEND);
     if (nx == ABSENT || !has_f(nx) || !in_window(bid)) { abort = true; return; }   // chain.rs:180-185 Err / window: step_kernel's business
 #pragma unroll
     for (int r = 0; r < R; ++r)
@@ -384,12 +481,14 @@ struct SymGroup {
     cache_put(F0, bid, nx, tk);
     if (bid > fmaxkey) fmaxkey = bid;
     fhead = bid;                                           // chain.rs:188-190: unconditionally
+    phase(outer);
   }
   __device__ __forceinline__ void follower_tick(const SymMail& in, SymMail& out) {
     if (in.hb) follower_heartbeat(in, out);
     if (in.ae) {                                           // follower.rs:130-176 with voted_for == Some(leader)
+      phase(SP_SCAN);
       for (uint32_t k = 0; k < in.ae_nb && !abort; ++k) {
-        const uint32_t bid = in.ae_id[k];
+        const uint32_t bid = in.id(k);
         uint32_t nx; uint64_t tk;
         fetch_sent(bid, in.mk, n_app, nx, tk);             // the block as the leader sent it
         follower_extend(bid, nx, tk);
@@ -409,6 +508,7 @@ struct SymGroup {
   __device__ __forceinline__ void follower_tick_view(const SymMail& in, uint32_t phf, uint32_t modef, uint32_t mk, SymMail& out) {
     if (in.hb) follower_heartbeat(in, out);
     if (!in.ae || abort) return;
+    phase(SP_SCAN);
     const uint32_t take = modef ? JR_MAX_AE_BLOCKS : 1u;
     uint32_t bid = max(phf, tbase), pulled = 0, nb = 0;
     while (pulled < 1 + take) {
@@ -577,7 +677,7 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, SPLIT>& s, SymMail& m, con
             uint32_t nx; uint64_t tk;
             s.fetch(L, bu.x, nx, tk);                       // the sim re-reads the block from the leader's table: must be what was sent
             if (nx != bu.y || tk != ((uint64_t)bu.z | ((uint64_t)bu.w << 32))) return false;
-            m.ae_id[k] = bu.x;
+            m.set_id(k, bu.x);
           }
           u += 1 + nb;
         } else {                                            // the others point at it
@@ -674,9 +774,10 @@ __device__ __forceinline__ void sym_leave_leader(SymGroup<R, SPLIT>& s, const Sy
           first = u + 1;
           put(u, make_uint4(unit_hdr(JR_CMD_APPEND_ENTRIES, 0, last.ae_nb, r + 1), (uint32_t)s.term, (uint32_t)(s.term >> 32), first));
           for (uint32_t k = 0; k < last.ae_nb; ++k) {
+            const uint32_t bid = last.id(k);
             uint32_t nx; uint64_t tk;
-            s.fetch(L, last.ae_id[k], nx, tk);
-            put(first + k, make_uint4(last.ae_id[k], nx, (uint32_t)tk, (uint32_t)(tk >> 32)));
+            s.fetch(L, bid, nx, tk);
+            put(first + k, make_uint4(bid, nx, (uint32_t)tk, (uint32_t)(tk >> 32)));
           }
           u += 1 + last.ae_nb;
           have = true;
@@ -829,6 +930,12 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.rows = smem + gi;
   s.enc = smem + 2 * SYM_ROWS * S + gi;
   uint4* mail = smem + SYM_SMEM_UNITS * S + gi;            // [k * S]: k = 2 * buf + {0, 1} leader -> followers, 4 + buf followers -> leader
+#ifdef JR_PROFILE
+  for (uint32_t i = threadIdx.x; i < 8 * 3 * 16 * 2; i += blockDim.x) jr_prof_smem()[i] = 0;
+  s.prole = lead ? JR_ROLE_LEADER : JR_ROLE_FOLLOWER;
+  s.pslot = SP_ENTER;
+  s.pt = clock64();
+#endif
   s.cache_clear(lead ? 0u : SYM_ROWS, SYM_ROWS);
   const uint32_t blk = g / GROUPS_PER_CTA;                  // step_kernel's 32-group block of this warp pair
   if (lead && lane == 0 && g < d.Gp) symblk[blk] = 1;      // (cleared below by any lane whose group is not folded)
@@ -836,6 +943,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   SymMail a;
   bool dead = !sym_enter(s, a, p, 1 - p.cur);
   pair_sync();                                         // the other lane's sym_enter may still be reading this lane's (empty) cache
+  s.phase(SP_FILL);
   if (!dead) {
     if (lead) {
       s.cache_fill(s.L, s.maxkey);
@@ -861,6 +969,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.now = p.now;
   uint32_t cur = 0;                                        // mail buffer written this tick; 1 - cur is read
   for (uint32_t t = 0; t < p.n_ticks; ++t) {
+    s.phase(SP_MAIL_IN);
     if (lead && (JR_SYM2_ROLES & 1)) {
       if (!dead) {
         const uint4 c = mail[(4 + (1 - cur)) * S];
@@ -908,6 +1017,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
           } else {
             s.follower_tick_view(in, ma.w, (ma.x & SYM2_MODE) ? 1u : 0u, ma.z, out);
           }
+          s.phase(SP_MAIL_OUT);
           if (s.abort) dead = true;
           else mail[(4 + cur) * S] = make_uint4(out.hbr | (out.hbr_has << 1) | (out.ar << 2), out.hbr_commit, out.ar_head, 0u);
         }
@@ -915,9 +1025,11 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
       if (dead) mail[(4 + cur) * S] = make_uint4(SYM2_ABORT, 0u, 0u, 0u);
     }
     s.now += p.dt;
+    s.phase(SP_BARRIER);
     pair_sync();
     cur ^= 1u;
   }
+  s.phase(SP_LEAVE);
   const uint32_t lastb = cur ^ 1u;                         // the buffers the last tick wrote
   const uint4 la = mail[(2 * lastb) * S], lc = mail[(4 + lastb) * S];
   const bool ok = !dead && !((la.x | lc.x) & SYM2_ABORT);
@@ -935,6 +1047,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
       sym_leave_followers(s, last, cur_last);
     }
   }
+  s.phase(SP_TRUNC);
   if (p.trunc) {   // jr_truncate(margin) for this group (truncate_kernel, engine.cu): every replica is live, the
     //              leader's commit after the last tick travels in its last mail
     pair_sync();   // the leader lane's sym_leave may still be reading rows this is about to blank
@@ -956,6 +1069,15 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
       if (g < d.G) *(volatile uint32_t*)d.hunf = p.epoch;   // advisory, for the host's choice of the next step_kernel grid
     }
   }
+#ifdef JR_PROFILE
+  s.phase(SP_TRUNC);
+  __syncthreads();
+  if (d.prof)
+    for (uint32_t i = threadIdx.x; i < 4 * 3 * 16 * 2; i += blockDim.x) {
+      const unsigned long long v = jr_prof_smem()[i];
+      if (v) atomicAdd(d.prof + (i % (3 * 16 * 2)), v);
+    }
+#endif
 }
 
 // symblk[b] = every group of 32-group block b was folded (step_kernel CTAs of such blocks return at once)
