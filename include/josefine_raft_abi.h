@@ -25,6 +25,7 @@
  *   jr_fsm_records_*   <- the receiving end of fsm_tx         src/raft/fsm.rs:52-56 (Driver::run's rx.recv loop),
  *                         fed by leader.rs:87-99,177-197 and follower.rs:198-207; compact form, see jr_fsm_record
  *   jr_fsm_expand      <- Instruction::{Apply,Notify}         src/raft/fsm.rs:19-29, one per record element
+ *   jr_fsm_responses   <- fsm::Driver's notification map and the ClientResponse it sends  src/raft/fsm.rs:57-81
  *   jr_node_restart    <- RaftHandle::new over an existing data directory: Chain::new reopening a
  *                         persisted chain                     src/raft/chain.rs:117-137
  *   jr_node_restart_many <- RaftHandle::new over many existing data directories (one per (group, node)) in one call
@@ -86,6 +87,8 @@ extern "C" {
 #define JR_MAX_AE_BLOCKS 5u       /* MAX_INFLIGHT, src/raft/progress.rs:117          */
 #define JR_MAX_NODE_ID 65534u     /* deviation D4                                    */
 #define JR_CLIENT_QUEUE_CAP 4u    /* queued_reqs bound per replica (reference: Vec)  */
+#define JR_NOTIFY_RUNS 8u         /* pending-notification runs per replica with JR_F_CLIENT_RESPONSES
+                                   * (reference: the Driver's unbounded HashMap, fsm.rs:36,78-81) */
 
 /* ---- status codes (API misuse / resources; never consensus outcomes) ---- */
 typedef enum jr_status {
@@ -149,8 +152,10 @@ enum {
   JR_F_CAPTURE_MESSAGES = 1u << 1,       /* jr_step may return every emitted Message (rpc_rx) */
   JR_F_CAPTURE_FSM = 1u << 2,            /* Instructions are stored (jr_step / jr_drain_fsm)  */
   JR_F_STREAM_DIGEST = 1u << 3,          /* keep the running digests jr_stream_digest returns  */
-  JR_F_NO_SYMMETRIC_FOLD = 1u << 4       /* jr_run* never take the symmetric-group fast path (DESIGN.md section 3b); results are
+  JR_F_NO_SYMMETRIC_FOLD = 1u << 4,      /* jr_run* never take the symmetric-group fast path (DESIGN.md section 3b); results are
                                           * identical either way -- the flag exists for A/B measurements and tests      */
+  JR_F_CLIENT_RESPONSES = 1u << 5        /* every drain also runs fsm::Driver's notification map on the device and returns the
+                                          * ClientResponses it produces (jr_fsm_responses).  Requires JR_F_CAPTURE_FSM */
 };
 
 /* ---- configuration (RaftConfig, src/raft/config.rs:14-41, batched) --------- */
@@ -250,8 +255,12 @@ typedef struct jr_fsm_instr {
  *                    reproduce its stream exactly (jr_fsm_expand does).
  * A steady-state follower needs one APPLY record per launch, a leader one APPLY + one NOTIFY + one PATTERN per
  * 160 Instructions, whatever the number of fused ticks -- when tokens advance by a constant stride.
+ *   JR_FSMR_RESPONSE (jr_fsm_responses only, never in a record batch) `count` ClientResponses that replica's
+ *                    fsm::Driver sent (fsm.rs:66-76): element i answers the request whose block id0+i it just applied,
+ *                    to address (addr >> 16, addr & 0xffff) as the Notify gave it, with request token tok0 + i*stride.
+ *                    count == 1 is the general case (stride 0).
  */
-enum { JR_FSMR_APPLY = 0, JR_FSMR_NOTIFY = 1, JR_FSMR_PATTERN = 2 };
+enum { JR_FSMR_APPLY = 0, JR_FSMR_NOTIFY = 1, JR_FSMR_PATTERN = 2, JR_FSMR_RESPONSE = 3 };
 typedef struct jr_fsm_record {
   uint32_t group;
   uint32_t hdr;      /* bits 0-1 JR_FSMR_*, bits 2-4 node id - 1, bits 8-31 count */
@@ -444,6 +453,26 @@ jr_status jr_drain_fsm(jr_engine* e, jr_fsm_instr* out, size_t cap, size_t* n);
  */
 jr_status jr_fsm_records_async(jr_engine* e);
 jr_status jr_fsm_records_wait(jr_engine* e, const jr_fsm_record** records, jr_fsm_batch* batch);
+/*
+ * With JR_F_CLIENT_RESPONSES: the ClientResponses of the batch most recently taken on this engine (by
+ * jr_fsm_records_wait, jr_drain_fsm -- also with out == NULL -- or jr_step with out_fsm), as JR_FSMR_RESPONSE runs
+ * sorted by (node, group), FIFO per replica.  batch->n_records = runs, n_instructions = ClientResponses they stand for,
+ * n_dropped = notifications and responses the engine could not hold, node_offset as for records.  Same buffer lifetime
+ * and thread as jr_fsm_records_wait.
+ * Per replica the device runs fsm::Driver (fsm.rs:57-81) over exactly the Instructions that leave the engine through a
+ * drain: Notify{block_id, id, address} inserts block_id -> (address, id); Apply{block} of a block other than 0 removes
+ * block.id and, if it was there, answers.  Matching is by block id only, as in the reference (DESIGN.md N5).
+ * jr_node_restart / _many give the replica a new, empty map (a new process gets a new Driver, server.rs:80-81, fsm.rs:48)
+ * from that point of its Instruction stream on: its undrained Instructions from before the restart are still drained
+ * and go through the old map.  jr_engine_reset empties every map; save / restore carry them.
+ * Limits never produce a wrong answer, only a missing one: a notification that does not fit in JR_NOTIFY_RUNS runs
+ * evicts the oldest run; a replica whose batch lost records (or whose records did not all fit in the batch buffer)
+ * clears its map and answers nothing from that batch; with three or more restarts of a replica between two drains,
+ * the Instructions between its first and last restart are not matched.  All of these count in n_dropped (as do
+ * responses that did not fit, one per response) and make the call return JR_E_CAPACITY (runs still returned).  JR_E_INVAL without the flag or
+ * before the first batch.
+ */
+jr_status jr_fsm_responses(jr_engine* e, const jr_fsm_record** responses, jr_fsm_batch* batch);
 /*
  * Pure host function (no device, no engine): records (any order across replicas, FIFO per replica) ->
  * Instructions, group-major, node ascending, FIFO per node.  out may be NULL to size the buffer.

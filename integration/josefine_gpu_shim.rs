@@ -182,6 +182,8 @@ extern "C" {
     #[allow(dead_code)]
     fn jr_fsm_records_wait(e: *mut c_void, records: *mut *const c_void, batch: *mut c_void) -> c_int;
     #[allow(dead_code)]
+    fn jr_fsm_responses(e: *mut c_void, responses: *mut *const JrFsmRecord, batch: *mut c_void) -> c_int;
+    #[allow(dead_code)]
     fn jr_chain_export_many(e: *mut c_void, groups: *const u32, nodes: *const u32, n: usize, out: *mut JrPersistedChain,
                             blocks: *mut JrBlock, cap_blocks: usize, n_blocks: *mut usize) -> c_int;
     #[allow(dead_code)]
@@ -222,6 +224,45 @@ unsafe fn restart_hosted_groups(engine: *mut c_void, id: u32, now_ms: u64, trees
         blocks.extend_from_slice(bl);
     }
     jr_node_restart_many(engine, now_ms, chains.as_ptr(), chains.len(), blocks.as_ptr(), blocks.len())
+}
+
+/// jr_fsm_record (32 B); with JR_FSMR_RESPONSE (kind 3) element i answers request token tok0 + i*stride.
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct JrFsmRecord {
+    pub group: u32,
+    pub hdr: u32, // bits 0-1 kind, 2-4 node id - 1, 8-31 count
+    pub id0: u32,
+    pub addr: u32, // client_kind << 16 | client_id
+    pub tok0: u64,
+    pub stride: u64,
+}
+#[allow(dead_code)]
+const JR_F_CLIENT_RESPONSES: u32 = 1 << 5;
+
+/// Sketch: the `requests` map of server.rs:144-151 completed from the device's ClientResponse runs of the batch just
+/// taken (engine created with JR_F_CAPTURE_FSM | JR_F_CLIENT_RESPONSES, after jr_fsm_records_wait).  Address::Client
+/// completes a local request; Address::Peer(n) is a proxied one the host relays to node n as Command::ClientResponse
+/// (follower.rs:271-282).  `complete(group, token)` takes the oneshot out of `requests` and sends Ok(..) on it.
+#[allow(dead_code)]
+unsafe fn answer_clients(engine: *mut c_void, mut complete: impl FnMut(u32, u64), mut relay: impl FnMut(u32, u32, u64)) -> c_int {
+    let mut runs: *const JrFsmRecord = std::ptr::null();
+    let mut batch = [0u64; 8]; // jr_fsm_batch: n_records, n_dropped, n_instructions, node_offset[9], reserved
+    let st = jr_fsm_responses(engine, &mut runs, batch.as_mut_ptr() as *mut c_void);
+    if st != 0 && st != 4 {
+        return st; // JR_E_CAPACITY (4): some requests stay unanswered (engine limits), the runs are still valid
+    }
+    for k in 0..batch[0] as usize {
+        let r = &*runs.add(k);
+        for i in 0..(r.hdr >> 8) as u64 {
+            let token = r.tok0.wrapping_add(i.wrapping_mul(r.stride));
+            match (r.addr >> 16) as u8 {
+                A_PEER => relay(r.group, r.addr & 0xFFFF, token),
+                _ => complete(r.group, token),
+            }
+        }
+    }
+    st
 }
 
 // Command discriminants, in the order of `enum Command` (src/raft/mod.rs:160-227)

@@ -12,6 +12,7 @@ MAX_REPLICAS = 8
 MAX_AE_BLOCKS = 5
 MAX_NODE_ID = 65534
 CLIENT_QUEUE_CAP = 4
+NOTIFY_RUNS = 8           # JR_NOTIFY_RUNS: pending-notification runs per replica (F_CLIENT_RESPONSES)
 
 # jr_status
 OK, E_INVAL, E_NOMEM, E_CUDA, E_CAPACITY, E_UNKNOWN_NODE, E_NO_DEVICE = range(7)
@@ -50,6 +51,7 @@ F_CAPTURE_MESSAGES = 1 << 1
 F_CAPTURE_FSM = 1 << 2
 F_STREAM_DIGEST = 1 << 3
 F_NO_SYMMETRIC_FOLD = 1 << 4
+F_CLIENT_RESPONSES = 1 << 5
 
 # step flags
 STEP_DELIVER = 1 << 0
@@ -136,7 +138,7 @@ class ReplicaState(C.Structure):
         return d
 
 
-FSMR_APPLY, FSMR_NOTIFY, FSMR_PATTERN = 0, 1, 2
+FSMR_APPLY, FSMR_NOTIFY, FSMR_PATTERN, FSMR_RESPONSE = 0, 1, 2, 3
 
 
 class FsmRecord(C.Structure):
@@ -188,7 +190,7 @@ ENGINE_SYMBOLS = [
     "jr_last_error", "jr_config_default", "jr_step", "jr_run", "jr_run_proposals", "jr_run_tokens", "jr_run_token_runs", "jr_drain_fsm", "jr_query",
     "jr_chain_read", "jr_state_digest", "jr_stream_digest", "jr_fault_count", "jr_fold_count", "jr_compact",
     "jr_set_alive", "jr_kill_leaders", "jr_leader_table_device", "jr_leader_table", "jr_leader_table_async", "jr_leader_table_wait",
-    "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
+    "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_responses", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
     "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
 ]
 

@@ -564,7 +564,10 @@ __global__ void export_pack_kernel(const Dev d, const jr_persisted_chain* desc, 
 // request k = reqs[k].  Host-validated: distinct replicas; ids strictly ascending inside [floor, floor + cap).  From host
 // data the window is emptied (an empty sled tree) and refilled; JR_RESTART_IN_PLACE keeps the rows and takes commit and
 // the commit key from the replica's own P2 -- the tree as the old incarnation left it.
-__global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persisted_chain* reqs, uint32_t n, const jr_block* blocks) {
+// rm (JR_F_CLIENT_RESPONSES, else null): the new process's fsm::Driver starts with an empty map (server.rs:80-81, fsm.rs:48)
+// from this point of the replica's Instruction stream on; the next drain's fsm_respond_kernel clears the map there.
+__global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persisted_chain* reqs, uint32_t n, const jr_block* blocks,
+                                    uint4* rm) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const jr_persisted_chain q = reqs[k];
@@ -604,6 +607,21 @@ __global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persiste
   d.mk[i] = mk;
   d.oc[0][i] = 0;
   d.oc[1][i] = 0;
+  if (rm) {
+    const uint32_t pos = d.fc[i].y;
+    uint4 m = rm[i];
+    if (!m.z) m.x = pos;
+    m.y = pos;
+    m.z = min(m.z + 1u, 3u);
+    rm[i] = m;
+  }
+}
+
+// jr_step starts every replica's Instruction FIFO afresh: the Instructions before a pending restart are gone, so the map
+// is cleared at the start of the new stream.
+__global__ void restart_marks_rebase_kernel(const Dev d, uint4* rm) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < (size_t)d.R * d.Gp && rm[i].z) rm[i] = make_uint4(0u, 0u, 1u, 0u);
 }
 
 // ---- Instruction-stream drain -----------------------------------------------------------------
@@ -616,26 +634,29 @@ struct FsmHeader {          // written by fsm_pack_kernel next to the records
   unsigned long long n_records, n_dropped, n_instructions;
   uint32_t node_offset[JR_MAX_REPLICAS + 1];
   uint32_t ready;           // epoch of the batch, written last
+  unsigned long long n_wanted;   // records the FIFOs held, before the cut at the batch's capacity
 };
 
 // Three small kernels (CTAs of T threads; the CPU emulation runs them with T = 1):
 //   fsm_count_kernel  per-CTA sums of the replicas' record counts            -> part[3][n_ctas]
 //   fsm_scan_kernel   one CTA: exclusive scan of those sums, batch totals     -> part[0] becomes CTA offsets, hdr
 //   fsm_pack_kernel   CTA-local scan + CTA offset = each replica's position; copies its records, empties its FIFO
-// Padded groups (g >= G) contribute nothing.
+// Padded groups (g >= G) contribute nothing.  The same three pack the client responses (JR_F_CLIENT_RESPONSES): they
+// work on the FIFO, counts {stored, elements} and staging they are given, F runs per replica either way.
 __device__ __forceinline__ uint32_t fsm_kept(const Dev& d, size_t i, uint2 c) {
   return (uint32_t)(i % d.Gp) < d.G ? min(c.x, d.F) : 0u;
 }
 
-__global__ void fsm_count_kernel(const Dev d, unsigned long long* part, uint32_t n_ctas) {
+// `xdrop` (may be null): elements each replica lost besides the runs beyond F.
+__global__ void fsm_count_kernel(const Dev d, const uint2* cnt, const uint32_t* xdrop, unsigned long long* part, uint32_t n_ctas) {
   __shared__ unsigned long long s[3][SCAN_THREADS / 32];
   const size_t plane = (size_t)d.R * d.Gp;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   unsigned long long rec = 0, drop = 0, ins = 0;
   if (i < plane && (uint32_t)(i % d.Gp) < d.G) {
-    const uint2 c = d.fc[i];
+    const uint2 c = cnt[i];
     rec = min(c.x, d.F);
-    drop = c.x > d.F ? c.x - d.F : 0u;
+    drop = (c.x > d.F ? c.x - d.F : 0u) + (xdrop ? xdrop[i] : 0u);
     ins = c.y;
   }
 #ifdef JR_EMU
@@ -657,7 +678,9 @@ __global__ void fsm_count_kernel(const Dev d, unsigned long long* part, uint32_t
   part[2 * (size_t)n_ctas + blockIdx.x] = ins;
 }
 
-__global__ void fsm_scan_kernel(unsigned long long* part, uint32_t n_ctas, FsmHeader* hdr, uint32_t cap_records) {
+// elem_drops: records cut off by cap_records are counted by their elements, in fsm_pack_kernel (the client responses: their
+// n_dropped counts responses), instead of one each here.
+__global__ void fsm_scan_kernel(unsigned long long* part, uint32_t n_ctas, FsmHeader* hdr, uint32_t cap_records, bool elem_drops) {
   __shared__ unsigned long long s_sum[SCAN_THREADS];
   const uint32_t t = threadIdx.x, T = blockDim.x;
   const uint32_t per = (n_ctas + T - 1) / T;
@@ -671,7 +694,8 @@ __global__ void fsm_scan_kernel(unsigned long long* part, uint32_t n_ctas, FsmHe
     unsigned long long run = 0;
     for (uint32_t k = 0; k < T; ++k) { const unsigned long long v = s_sum[k]; s_sum[k] = run; run += v; }
     hdr->n_records = min(run, (unsigned long long)cap_records);
-    hdr->n_dropped = run > cap_records ? run - cap_records : 0ull;   // + the per-replica drops, added below
+    hdr->n_dropped = run > cap_records && !elem_drops ? run - cap_records : 0ull;   // + the per-replica drops, added below
+    hdr->n_wanted = run;
     hdr->n_instructions = 0;
   }
   __syncthreads();
@@ -696,7 +720,8 @@ __global__ void fsm_scan_kernel(unsigned long long* part, uint32_t n_ctas, FsmHe
       s_warp[lane] = wi - mine;                           // exclusive prefix of the warp totals
       if (lane == 31) {
         hdr->n_records = min(wi, (unsigned long long)cap_records);
-        hdr->n_dropped = wi > cap_records ? wi - cap_records : 0ull;   // + the per-replica drops, added below
+        hdr->n_dropped = wi > cap_records && !elem_drops ? wi - cap_records : 0ull;   // + the per-replica drops, added below
+        hdr->n_wanted = wi;
         hdr->n_instructions = 0;
       }
     }
@@ -717,11 +742,12 @@ __global__ void fsm_scan_kernel(unsigned long long* part, uint32_t n_ctas, FsmHe
 }
 
 // Thread i moves its replica's records to out[position ..] and empties the FIFO.  `out` may be mapped host memory.
-__global__ void fsm_pack_kernel(const Dev d, const unsigned long long* part, FsmHeader* hdr, uint4* out, uint32_t cap_records) {
+__global__ void fsm_pack_kernel(const Dev d, const uint4* fifo, uint2* cnt, const unsigned long long* part, FsmHeader* hdr,
+                                uint4* out, uint32_t cap_records, bool elem_drops) {
   __shared__ uint32_t s_warp[SCAN_THREADS / 32];
   const size_t plane = (size_t)d.R * d.Gp;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t n = i < plane ? fsm_kept(d, i, d.fc[i]) : 0u;
+  const uint32_t n = i < plane ? fsm_kept(d, i, cnt[i]) : 0u;
   // exclusive scan of n over the CTA
   uint32_t pre = 0;
 #ifdef JR_EMU
@@ -743,13 +769,232 @@ __global__ void fsm_pack_kernel(const Dev d, const unsigned long long* part, Fsm
   if (i < plane) {
     const uint32_t at = (uint32_t)min(at64, (unsigned long long)cap_records);
     for (uint32_t k = 0; k < n && at + k < cap_records; ++k) {
-      out[(size_t)2 * (at + k)] = d.fs[(size_t)(2 * k) * plane + i];
-      out[(size_t)2 * (at + k) + 1] = d.fs[(size_t)(2 * k + 1) * plane + i];
+      out[(size_t)2 * (at + k)] = fifo[(size_t)(2 * k) * plane + i];
+      out[(size_t)2 * (at + k) + 1] = fifo[(size_t)(2 * k + 1) * plane + i];
+    }
+    if (elem_drops && at + n > cap_records) {   // (rare: the batch buffer is full)
+      unsigned long long lost = 0;
+      for (uint32_t k = cap_records > at ? cap_records - at : 0u; k < n; ++k) lost += fifo[(size_t)(2 * k) * plane + i].y >> 8;
+      atomicAdd(&hdr->n_dropped, lost);
     }
     if (i % d.Gp == 0) hdr->node_offset[i / d.Gp] = at;
     if (i + 1 == plane) hdr->node_offset[d.R] = (uint32_t)min(at64 + n, (unsigned long long)cap_records);
-    d.fc[i] = make_uint2(0, 0);
+    cnt[i] = make_uint2(0, 0);
   }
+}
+
+// ---- Client responses (JR_F_CLIENT_RESPONSES): fsm::Driver's notification map on the device ---------------------------
+// fsm.rs:57-81 per replica: Notify{block_id, id, address} inserts block_id -> (address, id) (HashMap insert: it
+// overwrites); Apply{block} skips block 0 (fsm.rs:61-63), otherwise notifications.remove(block.id) and a hit sends
+// ClientResponse{id} to the address (fsm.rs:66-76).  Matching is by block id only (DESIGN.md N5).
+// The map lives in the PN plane as at most JR_NOTIFY_RUNS runs per replica, oldest first: run = ids id0 .. id0+count-1,
+// one address, request tokens tok0 + k*stride.  Steady state is one run of two or three ids.
+struct RespPlanes {
+  uint4* pn;        // [2*run + half][replica][group]: {id0, count, addr, 0}, {tok0 lo, hi, stride lo, hi}
+  uint32_t* pnc;    // [replica][group]: runs held
+  uint4* rs;        // this drain's response runs, jr_fsm_record layout, F per replica: [2*k + half][replica][group]
+  uint2* rc;        // [replica][group]: {runs stored, responses they stand for}
+  uint32_t* rd;     // [replica][group]: notifications and responses dropped by this drain
+  uint4* rm;        // [replica][group]: restarts since the last drain {stream position of the first, of the last, count <= 3}
+};
+
+// 16-byte units of the PN allocation: runs, run counts (u32, padded), restart marks
+inline size_t pn_units(size_t plane) { return 2 * (size_t)JR_NOTIFY_RUNS * plane + (plane + 3) / 4 + plane; }
+
+struct PnRun {
+  uint32_t id0, count, addr;
+  unsigned long long tok0, stride;
+};
+
+// The walk follows jr_fsm_expand: a replica's Apply stream is the masked APPLY records naming it (any replica's FIFO,
+// ascending FIFO, in front) and then its own unmasked APPLY records; its Notify stream is its own NOTIFY records; its
+// PATTERN records place the Notifies.  One thread per replica; the FIFOs are only read (the pack that empties them runs
+// after this kernel).  A replica whose batch lost records -- own FIFO full, a masked record lost in a peer's FIFO (the
+// records it can see stand for fewer Instructions than it emitted) or a full batch buffer -- clears its map instead.
+// Restarts (rm): a restarted replica's undrained Instructions are still drained, but they belong to the old process's
+// Driver, whose map dies with it (server.rs:80-81, fsm.rs:48).  The walk clears the map at the stream position where the
+// restart happened: what came before went through the old map, what comes after goes through the new one.  Two restarts
+// in one drain are exact as well; with three or more, the Instructions between the first and the last restart are not
+// matched at all (their Notifies count as dropped).
+__global__ void fsm_respond_kernel(const Dev d, const RespPlanes q, const FsmHeader* hdr, uint32_t cap_records) {
+  const size_t plane = (size_t)d.R * d.Gp;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= plane) return;
+  const uint32_t r = (uint32_t)(i / d.Gp), g = (uint32_t)(i % d.Gp);
+  q.rc[i] = make_uint2(0u, 0u);
+  q.rd[i] = 0u;
+  if (g >= d.G) return;
+  const uint4 m = q.rm[i];
+  if (m.z) q.rm[i] = make_uint4(0u, 0u, 0u, 0u);
+  const uint2 c = d.fc[i];
+  const uint32_t own = min(c.x, d.F);
+  uint32_t n = q.pnc[i];
+  bool notifies = false;
+  for (uint32_t k = 0; k < own && !notifies; ++k) notifies = (d.fs[(size_t)(2 * k) * plane + i].y & 3u) == FSR_NOTIFY;
+  if (n == 0 && !notifies) return;   // nothing to match, nothing to insert: every steady-state follower
+  auto rec_hdr = [&](uint32_t src, uint32_t k) { return d.fs[(size_t)(2 * k) * plane + (size_t)src * d.Gp + g]; };
+  auto u64 = [](uint32_t lo, uint32_t hi) { return (unsigned long long)lo | ((unsigned long long)hi << 32); };
+  auto kept =[&](uint32_t src) { return min(d.fc[(size_t)src * d.Gp + g].x, d.F); };
+  auto mine = [&](uint32_t src_phase, uint4 h) {   // src_phase < R: masked phase over FIFO src_phase; == R: own records
+    const bool apply = (h.y & 3u) == FSR_APPLY;
+    return src_phase < d.R ? (apply && h.w != 0u && ((h.w >> r) & 1u)) : (apply && h.w == 0u);
+  };
+  PnRun t[JR_NOTIFY_RUNS + 1];
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint4 a = q.pn[(size_t)(2 * k) * plane + i], b = q.pn[(size_t)(2 * k + 1) * plane + i];
+    t[k] = PnRun{a.x, a.y, a.z, u64(b.x, b.y), u64(b.z, b.w)};
+  }
+  uint32_t drop = 0;
+  // Instructions the visible records stand for
+  unsigned long long seen = 0;
+  for (uint32_t src = 0; src <= d.R; ++src) {
+    const uint32_t from = src < d.R ? src : r, m = kept(from);
+    for (uint32_t k = 0; k < m; ++k) {
+      const uint4 h = rec_hdr(from, k);
+      if (mine(src, h) || (src == d.R && (h.y & 3u) == FSR_NOTIFY)) seen += h.y >> 8;
+    }
+  }
+  if (c.x > d.F || seen != c.y || hdr->n_wanted > cap_records) {
+    for (uint32_t k = 0; k < n; ++k) drop += t[k].count;
+    q.pnc[i] = 0u;
+    q.rd[i] = drop;
+    return;
+  }
+  auto erase = [&](uint32_t k) {
+    for (uint32_t j = k; j + 1 < n; ++j) t[j] = t[j + 1];
+    --n;
+  };
+  auto fit = [&]() {   // over JR_NOTIFY_RUNS: the oldest run goes
+    if (n > JR_NOTIFY_RUNS) { drop += t[0].count; erase(0); }
+  };
+  auto find = [&](uint32_t id) {
+    uint32_t k = 0;
+    while (k < n && id - t[k].id0 >= t[k].count) ++k;
+    return k;
+  };
+  // notifications.remove(id) of the entry known to sit in run k: its address and request token
+  auto take = [&](uint32_t k, uint32_t id, uint32_t& addr, unsigned long long& tok) {
+    PnRun& x = t[k];
+    const uint32_t off = id - x.id0;
+    addr = x.addr;
+    tok = x.tok0 + (unsigned long long)off * x.stride;
+    if (x.count == 1u) {
+      erase(k);
+    } else if (off == 0u) {
+      x.id0 += 1u; x.tok0 += x.stride; x.count -= 1u;
+    } else if (off == x.count - 1u) {
+      x.count -= 1u;
+    } else {   // split: the ids above `id` become a run of their own, just as old
+      const PnRun y{id + 1u, x.count - off - 1u, x.addr, x.tok0 + (unsigned long long)(off + 1u) * x.stride, x.stride};
+      x.count = off;
+      for (uint32_t j = n; j > k + 1u; --j) t[j] = t[j - 1u];
+      t[k + 1u] = y;
+      ++n;
+      fit();
+    }
+  };
+  // response runs of this drain: the open one extends while block ids, address and tokens continue it
+  PnRun o{0u, 0u, 0u, 0ull, 0ull};
+  uint32_t n_runs = 0, n_resp = 0;
+  auto close = [&]() {
+    if (!o.count) return;
+    if (n_runs < d.F) {
+      q.rs[(size_t)(2 * n_runs) * plane + i] = make_uint4(g, JR_FSMR_RESPONSE | (r << 2) | (o.count << 8), o.id0, o.addr);
+      const unsigned long long st = o.count > 1u ? o.stride : 0ull;
+      q.rs[(size_t)(2 * n_runs + 1) * plane + i] =
+          make_uint4((uint32_t)o.tok0, (uint32_t)(o.tok0 >> 32), (uint32_t)st, (uint32_t)(st >> 32));
+      ++n_runs;
+      n_resp += o.count;
+    } else {
+      drop += o.count;
+    }
+    o.count = 0u;
+  };
+  // cursors: Apply (phase = source FIFO, then R = own records), Notify, PATTERN window
+  uint32_t a_src = 0, a_k = 0, a_e = 0, a_cnt = 0, a_id0 = 0;
+  uint32_t n_k = 0, n_e = 0, n_cnt = 0;
+  uint4 n_h = make_uint4(0u, 0u, 0u, 0u);
+  unsigned long long n_tok0 = 0, n_st = 0;
+  uint32_t p_k = 0, w0 = 0, wn = 0, wb2 = 0;
+  unsigned long long wb0 = 0, wb1 = 0;
+  for (uint32_t pos = 0; pos <= c.y; ++pos) {
+    if (m.z && (pos == m.x || pos == m.y)) n = 0u;   // a restart: the new process's Driver starts with an empty map
+    if (pos == c.y) break;
+    const bool skip = m.z > 2u && pos >= m.x && pos < m.y;
+    while (pos >= w0 + wn && p_k < own) {   // the next PATTERN window (they come in stream order)
+      const uint4 h = rec_hdr(r, p_k);
+      if ((h.y & 3u) == FSR_PATTERN) {
+        const uint4 v = d.fs[(size_t)(2 * p_k + 1) * plane + i];
+        w0 = h.z; wn = h.y >> 8; wb2 = h.w;
+        wb0 = u64(v.x, v.y);
+        wb1 = u64(v.z, v.w);
+      }
+      ++p_k;
+    }
+    const uint32_t b = pos - w0;
+    const bool note = pos >= w0 && b < wn && ((b < 64u ? wb0 >> b : b < 128u ? wb1 >> (b - 64u) : (unsigned long long)(wb2 >> (b - 128u))) & 1ull);
+    if (note) {
+      while (n_e >= n_cnt && n_k < own) {   // the next NOTIFY record of this replica
+        n_h = rec_hdr(r, n_k);
+        if ((n_h.y & 3u) == FSR_NOTIFY) {
+          const uint4 v = d.fs[(size_t)(2 * n_k + 1) * plane + i];
+          n_tok0 = u64(v.x, v.y);
+          n_st = u64(v.z, v.w);
+          n_cnt = n_h.y >> 8;
+          n_e = 0;
+        }
+        ++n_k;
+      }
+      if (n_e >= n_cnt) break;   // (a malformed stream; jr_fsm_expand rejects it too)
+      const uint32_t id = n_h.z + n_e, addr = n_h.w;
+      const unsigned long long tok = n_tok0 + (unsigned long long)n_e * n_st;
+      ++n_e;
+      if (skip) { ++drop; continue; }
+      const uint32_t k = find(id);   // insert overwrites (fsm.rs:80)
+      if (k < n) { uint32_t a2; unsigned long long t2; take(k, id, a2, t2); }
+      PnRun* last = n ? &t[n - 1u] : nullptr;
+      if (last && id == last->id0 + last->count && addr == last->addr && last->count < FS_MAX_RUN &&
+          (last->count == 1u || tok == last->tok0 + (unsigned long long)last->count * last->stride)) {
+        if (last->count == 1u) last->stride = tok - last->tok0;
+        last->count += 1u;
+      } else {
+        t[n++] = PnRun{id, 1u, addr, tok, 0ull};
+        fit();
+      }
+    } else {
+      while (a_e >= a_cnt && a_src <= d.R) {   // the next APPLY record of this replica's stream
+        const uint32_t from = a_src < d.R ? a_src : r;
+        if (a_k >= kept(from)) { ++a_src; a_k = 0; continue; }
+        const uint4 h = rec_hdr(from, a_k++);
+        if (mine(a_src, h)) { a_id0 = h.z; a_cnt = h.y >> 8; a_e = 0; }
+      }
+      if (a_e >= a_cnt) break;
+      const uint32_t id = a_id0 + a_e++;
+      if (id == 0u || skip) continue;   // fsm.rs:61-63
+      const uint32_t k = find(id);
+      if (k == n) continue;
+      uint32_t addr;
+      unsigned long long tok;
+      take(k, id, addr, tok);
+      if (o.count && id == o.id0 + o.count && addr == o.addr && o.count < FS_MAX_RUN &&
+          (o.count == 1u || tok == o.tok0 + (unsigned long long)o.count * o.stride)) {
+        if (o.count == 1u) o.stride = tok - o.tok0;
+        o.count += 1u;
+      } else {
+        close();
+        o = PnRun{id, 1u, addr, tok, 0ull};
+      }
+    }
+  }
+  close();
+  for (uint32_t k = 0; k < n; ++k) {
+    q.pn[(size_t)(2 * k) * plane + i] = make_uint4(t[k].id0, t[k].count, t[k].addr, 0u);
+    q.pn[(size_t)(2 * k + 1) * plane + i] = make_uint4((uint32_t)t[k].tok0, (uint32_t)(t[k].tok0 >> 32), (uint32_t)t[k].stride,
+                                                       (uint32_t)(t[k].stride >> 32));
+  }
+  q.pnc[i] = n;
+  q.rc[i] = make_uint2(n_runs, n_resp);
+  q.rd[i] = drop;
 }
 
 // Packed batch (device) -> the engine's pinned host buffer, by the SMs: the size is only known on the device, so
@@ -863,6 +1108,13 @@ struct jr_engine {
   std::mutex qmu;   // the two FIFOs of outstanding copy-outs (fsm_pending, tab_pending) and fsm_last_records: a second host thread may
                     // sit in jr_fsm_records_wait / jr_leader_table_wait while the first one keeps submitting
   uint32_t fsm_epoch = 0;
+  // client responses (JR_F_CLIENT_RESPONSES): packed into the second region of stage[b] / host[b] (resp_cap records from
+  // record fsm_cap on) with their header at fsm_stage_hdr[b][1] / fsm_host_hdr[b][1]
+  RespPlanes rp = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  uint32_t resp_cap = 0;
+  size_t resp_copied[NBUF] = {0, 0};
+  size_t resp_last = 0;                                       // size of the last response batch taken (the next copy's guess)
+  int resp_b = -1;                                            // buffer of the batch most recently taken (-1: none yet)
   // symmetric-group fold
   uint8_t* symdone = nullptr;   // device, Gp entries
   uint8_t* symblk = nullptr;    // device, Gp / 32 entries
@@ -1076,6 +1328,10 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
     set_err("fsm_units <= 2^20, 32 <= fsm_raw_units <= 2^20");
     return JR_E_INVAL;
   }
+  if ((cfg->flags & JR_F_CLIENT_RESPONSES) && !(cfg->flags & JR_F_CAPTURE_FSM)) {
+    set_err("JR_F_CLIENT_RESPONSES requires JR_F_CAPTURE_FSM");
+    return JR_E_INVAL;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     set_err("no CUDA device; this library has no CPU fallback");
@@ -1135,8 +1391,26 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
     const size_t want = cfg->fsm_host_records ? cfg->fsm_host_records
                                               : std::max(3 * reps + 1024, std::min<size_t>(reps * cfg->fsm_units, 1u << 16));
     e->fsm_cap = (uint32_t)std::min<size_t>(want, 0x7fffffffu);
+    if (d.flags & JR_F_CLIENT_RESPONSES) {
+      e->resp_cap = e->fsm_cap;
+      // PN runs, the run counts and the restart marks in one allocation: one checkpoint segment
+      uint4* pn = nullptr;
+      A(pn, pn_units(plane));
+      e->rp.pn = pn;
+      if (pn) {
+        e->rp.pnc = reinterpret_cast<uint32_t*>(pn + 2 * (size_t)JR_NOTIFY_RUNS * plane);
+        e->rp.rm = pn + 2 * (size_t)JR_NOTIFY_RUNS * plane + (plane + 3) / 4;
+      }
+      A(e->rp.rs, plane * 2 * (size_t)d.F);
+      A(e->rp.rc, plane);
+      A(e->rp.rd, plane);
+    }
+    const size_t n_hdr = e->resp_cap ? 2 : 1;
     A(e->fsm_part, 3 * plane);   // (sized for one-thread CTAs, which is what the CPU emulation launches)
-    for (int i = 0; i < jr_engine::NBUF; ++i) { A(e->fsm_stage[i], 2 * (size_t)e->fsm_cap); A(e->fsm_stage_hdr[i], 1); }
+    for (int i = 0; i < jr_engine::NBUF; ++i) {
+      A(e->fsm_stage[i], 2 * ((size_t)e->fsm_cap + e->resp_cap));
+      A(e->fsm_stage_hdr[i], n_hdr);
+    }
   }
   A(e->scratch, 8);
   A(d.scatter, 2);
@@ -1167,8 +1441,8 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
            cudaEventCreateWithFlags(&e->fsm_packed[i], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&e->fsm_landed[i], cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; ok && e->fsm_cap && i < jr_engine::NBUF; ++i)   // the drain's landing buffers: pinned, device-visible
-      ok = cudaHostAlloc((void**)&e->fsm_host[i], (size_t)e->fsm_cap * sizeof(jr_fsm_record), cudaHostAllocMapped) == cudaSuccess &&
-           cudaHostAlloc((void**)&e->fsm_host_hdr[i], sizeof(FsmHeader), cudaHostAllocMapped) == cudaSuccess;
+      ok = cudaHostAlloc((void**)&e->fsm_host[i], ((size_t)e->fsm_cap + e->resp_cap) * sizeof(jr_fsm_record), cudaHostAllocMapped) == cudaSuccess &&
+           cudaHostAlloc((void**)&e->fsm_host_hdr[i], (e->resp_cap ? 2 : 1) * sizeof(FsmHeader), cudaHostAllocMapped) == cudaSuccess;
     if (!ok) {
       set_err("copy streams / events could not be created");
       jr_engine_destroy(e);
@@ -1239,6 +1513,9 @@ jr_status jr_engine_reset(jr_engine* e) {
   CK(cudaMemsetAsync(d.done, 0, (size_t)(d.Gp / GROUPS_PER_CTA) * sizeof(uint32_t), e->stream));
   CK(cudaMemsetAsync(d.scatter, 0, 2 * sizeof(uint32_t), e->stream));   // [1] = the ticket counter: from here on only launches move it,
   e->ticket_sum = 0;                                                     //       and each one is told where it stands (ticket_base)
+  if (e->rp.pnc)   // every fsm::Driver map empty, no restart pending
+    CK(cudaMemsetAsync(e->rp.pnc, 0, ((plane + 3) / 4 + plane) * sizeof(uint4), e->stream));
+  e->resp_b = -1;
   JR_LAUNCH(init_kernel, (unsigned)((plane + 255) / 256), 256, e->stream, d);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -1377,11 +1654,12 @@ static jr_status capture_messages(jr_engine* e, int buf, std::vector<jr_msg>& ou
 static jr_status fsm_records_enqueue(jr_engine* e) {
   const Dev& d = e->d;
   if (!(d.flags & JR_F_CAPTURE_FSM)) { set_err("engine created without JR_F_CAPTURE_FSM"); return JR_E_INVAL; }
-  size_t last_records;
+  size_t last_records, last_resp;
   {
     std::lock_guard<std::mutex> l(e->qmu);
     if (e->fsm_npending == jr_engine::NBUF) { set_err("%d batches outstanding: call jr_fsm_records_wait first", jr_engine::NBUF); return JR_E_INVAL; }
     last_records = e->fsm_last_records;
+    last_resp = e->resp_last;
   }
   const int b = e->fsm_i;
   e->fsm_i = (b + 1) % jr_engine::NBUF;
@@ -1394,18 +1672,39 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
   const uint32_t T = 256, Ts = SCAN_THREADS;
 #endif
   const uint32_t n_ctas = (uint32_t)((plane + T - 1) / T);
-  JR_LAUNCH(fsm_count_kernel, n_ctas, T, e->stream, d, e->fsm_part, n_ctas);
+  JR_LAUNCH(fsm_count_kernel, n_ctas, T, e->stream, d, d.fc, nullptr, e->fsm_part, n_ctas);
   CK(cudaGetLastError());
-  JR_LAUNCH(fsm_scan_kernel, 1, Ts, e->stream, e->fsm_part, n_ctas, e->fsm_stage_hdr[b], e->fsm_cap);
+  JR_LAUNCH(fsm_scan_kernel, 1, Ts, e->stream, e->fsm_part, n_ctas, e->fsm_stage_hdr[b], e->fsm_cap, false);
   CK(cudaGetLastError());
-  JR_LAUNCH(fsm_pack_kernel, n_ctas, T, e->stream, d, e->fsm_part, e->fsm_stage_hdr[b], e->fsm_stage[b], e->fsm_cap);
+  if (e->resp_cap) {   // reads the FIFOs before the pack empties them
+    JR_LAUNCH(fsm_respond_kernel, n_ctas, T, e->stream, d, e->rp, e->fsm_stage_hdr[b], e->fsm_cap);
+    CK(cudaGetLastError());
+  }
+  JR_LAUNCH(fsm_pack_kernel, n_ctas, T, e->stream, d, d.fs, d.fc, e->fsm_part, e->fsm_stage_hdr[b], e->fsm_stage[b], e->fsm_cap,
+            false);
   CK(cudaGetLastError());
+  uint4* const resp_stage = e->fsm_stage[b] + 2 * (size_t)e->fsm_cap;
+  if (e->resp_cap) {
+    JR_LAUNCH(fsm_count_kernel, n_ctas, T, e->stream, d, e->rp.rc, e->rp.rd, e->fsm_part, n_ctas);
+    CK(cudaGetLastError());
+    JR_LAUNCH(fsm_scan_kernel, 1, Ts, e->stream, e->fsm_part, n_ctas, e->fsm_stage_hdr[b] + 1, e->resp_cap, true);
+    CK(cudaGetLastError());
+    JR_LAUNCH(fsm_pack_kernel, n_ctas, T, e->stream, d, e->rp.rs, e->rp.rc, e->fsm_part, e->fsm_stage_hdr[b] + 1, resp_stage,
+              e->resp_cap, true);
+    CK(cudaGetLastError());
+  }
   CK(cudaEventRecord(e->fsm_packed[b], e->stream));
   CK(cudaStreamWaitEvent(e->d2h, e->fsm_packed[b], 0));
   if (e->fsm_copy_by_sm) {
     JR_LAUNCH(fsm_copy_kernel, 32, 256, e->d2h, e->fsm_stage[b], e->fsm_stage_hdr[b], e->fsm_host[b], e->fsm_host_hdr[b], epoch);
     CK(cudaGetLastError());
     e->fsm_copied[b] = e->fsm_cap;
+    if (e->resp_cap) {
+      JR_LAUNCH(fsm_copy_kernel, 32, 256, e->d2h, resp_stage, e->fsm_stage_hdr[b] + 1, e->fsm_host[b] + 2 * (size_t)e->fsm_cap,
+                e->fsm_host_hdr[b] + 1, epoch);
+      CK(cudaGetLastError());
+      e->resp_copied[b] = e->resp_cap;
+    }
   } else {
     // Copy engine, speculatively: the batch size is only known on the device, so copy as many records as the previous
     // batch held plus a margin; fsm_records_take fetches the rest in the (rare) case the batch turned out larger.
@@ -1415,6 +1714,12 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
     if (guess) CK(cudaMemcpyAsync(e->fsm_host[b], e->fsm_stage[b], guess * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
     CK(cudaMemcpyAsync(e->fsm_host_hdr[b], e->fsm_stage_hdr[b], sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
     e->fsm_copied[b] = guess;
+    if (e->resp_cap) {   // the same scheme for the responses
+      const size_t rg = std::min<size_t>(e->resp_cap, std::max<size_t>(last_resp + last_resp / 8 + 1024, 16384));
+      CK(cudaMemcpyAsync(e->fsm_host[b] + 2 * (size_t)e->fsm_cap, resp_stage, rg * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
+      CK(cudaMemcpyAsync(e->fsm_host_hdr[b] + 1, e->fsm_stage_hdr[b] + 1, sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
+      e->resp_copied[b] = rg;
+    }
   }
   CK(cudaEventRecord(e->fsm_landed[b], e->d2h));
   e->fsm_used[b] = true;
@@ -1442,7 +1747,25 @@ static jr_status fsm_records_take(jr_engine* e, const jr_fsm_record** recs, jr_f
     CK(cudaEventSynchronize(e->fsm_landed[b]));
     e->fsm_copied[b] = h.n_records;
   }
-  { std::lock_guard<std::mutex> l(e->qmu); e->fsm_last_records = h.n_records; }
+  size_t n_resp = 0;
+  if (e->resp_cap) {
+    const FsmHeader& hr = e->fsm_host_hdr[b][1];
+    n_resp = hr.n_records;
+    if (hr.n_records > e->resp_copied[b]) {
+      const size_t have = e->resp_copied[b];
+      jr_fsm_record* dst = reinterpret_cast<jr_fsm_record*>(e->fsm_host[b] + 2 * (size_t)e->fsm_cap);
+      const jr_fsm_record* src = reinterpret_cast<const jr_fsm_record*>(e->fsm_stage[b] + 2 * (size_t)e->fsm_cap);
+      CK(cudaMemcpyAsync(dst + have, src + have, ((size_t)hr.n_records - have) * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
+      CK(cudaEventRecord(e->fsm_landed[b], e->d2h));
+      CK(cudaEventSynchronize(e->fsm_landed[b]));
+      e->resp_copied[b] = hr.n_records;
+    }
+  }
+  {
+    std::lock_guard<std::mutex> l(e->qmu);
+    e->fsm_last_records = h.n_records;
+    if (e->resp_cap) { e->resp_last = n_resp; e->resp_b = b; }
+  }
   if (recs) *recs = reinterpret_cast<const jr_fsm_record*>(e->fsm_host[b]);
   if (batch) {
     memset(batch, 0, sizeof *batch);
@@ -1544,6 +1867,11 @@ jr_status jr_step(jr_engine* e, jr_step_args* a) {
     CK(cudaStreamWaitEvent(e->stream, e->prop_ready[b], 0));
     p.proposals = e->prop[b];
     staged = b;
+  }
+  if (e->rp.rm) {   // PH_RESET_FSM below drops the undrained Instructions a pending restart mark points into
+    const size_t plane = (size_t)R * d.Gp;
+    JR_LAUNCH(restart_marks_rebase_kernel, (unsigned)((plane + 255) / 256), 256, e->stream, d, e->rp.rm);
+    CK(cudaGetLastError());
   }
   const uint32_t ph_first = PH_RESET_OUT | PH_RESET_FSM | ((a->flags & JR_STEP_DELIVER) ? PH_DRAIN : 0u);
   const uint32_t ph_last = ((p.proposals || p.n_synth) ? PH_PROPOSE : 0u) | ((a->flags & JR_STEP_TICK) ? PH_TICK : 0u);
@@ -1965,6 +2293,28 @@ jr_status jr_fsm_records_wait(jr_engine* e, const jr_fsm_record** records, jr_fs
   return fsm_records_take(e, records, batch);
 }
 
+jr_status jr_fsm_responses(jr_engine* e, const jr_fsm_record** responses, jr_fsm_batch* batch) {
+  if (!e) return JR_E_INVAL;
+  if (!e->resp_cap) { set_err("engine created without JR_F_CLIENT_RESPONSES"); return JR_E_INVAL; }
+  int b;
+  { std::lock_guard<std::mutex> l(e->qmu); b = e->resp_b; }
+  if (b < 0) { set_err("no batch has been taken yet"); return JR_E_INVAL; }
+  const FsmHeader& h = e->fsm_host_hdr[b][1];
+  if (responses) *responses = reinterpret_cast<const jr_fsm_record*>(e->fsm_host[b] + 2 * (size_t)e->fsm_cap);
+  if (batch) {
+    memset(batch, 0, sizeof *batch);
+    batch->n_records = h.n_records;
+    batch->n_dropped = h.n_dropped;
+    batch->n_instructions = h.n_instructions;
+    for (uint32_t r = 0; r <= JR_MAX_REPLICAS; ++r) batch->node_offset[r] = r <= e->d.R ? h.node_offset[r] : h.node_offset[e->d.R];
+  }
+  if (h.n_dropped) {
+    set_err("%llu notifications / responses were dropped (JR_NOTIFY_RUNS, fsm_units or lost records)", (unsigned long long)h.n_dropped);
+    return JR_E_CAPACITY;
+  }
+  return JR_OK;
+}
+
 // Pure host code: records -> Instructions (include/josefine_raft_abi.h, jr_fsm_record).
 jr_status jr_fsm_expand(const jr_fsm_record* recs, size_t n_records, uint32_t G, uint32_t R, jr_fsm_instr* out, size_t cap,
                         size_t* n_out) {
@@ -2344,7 +2694,7 @@ jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted
   CK(cudaMemcpyAsync(base, chains, n * sizeof(jr_persisted_chain), cudaMemcpyHostToDevice, e->stream));
   if (n_blocks) CK(cudaMemcpyAsync(base + o_blk, blocks, n_blocks * sizeof(jr_block), cudaMemcpyHostToDevice, e->stream));
   JR_LAUNCH(node_restart_kernel, (unsigned)((n + 127) / 128), 128, e->stream, d, now_ms, (const jr_persisted_chain*)base,
-            (uint32_t)n, (const jr_block*)(base + o_blk));
+            (uint32_t)n, (const jr_block*)(base + o_blk), e->rp.rm);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
   return JR_OK;
@@ -2394,6 +2744,8 @@ std::vector<Segment> save_segments(jr_engine* e) {
       {d.oc[0], plane * sizeof(uint32_t)}, {d.oc[1], plane * sizeof(uint32_t)},
       {d.fs, plane * ((d.flags & JR_F_CAPTURE_FSM) ? 2 * (size_t)d.F : 1) * sizeof(uint4)}, {d.fc, plane * sizeof(uint2)},
       {d.tb, (size_t)d.Gp * sizeof(uint32_t)}, {e->route, (size_t)d.G * sizeof(uint32_t)}};
+  if (e->rp.pn)   // the fsm::Driver maps (JR_F_CLIENT_RESPONSES only: other checkpoints keep their size and bytes)
+    v.push_back({e->rp.pn, pn_units(plane) * sizeof(uint4)});
   return v;
 }
 }  // namespace
@@ -2455,6 +2807,7 @@ jr_status jr_engine_restore(jr_engine* e, const void* buf, size_t bytes) {
   e->cur = (int)h.cur;
   e->step_index = h.step_index;
   e->fsm_npending = 0;
+  e->resp_b = -1;
   return JR_OK;
 }
 

@@ -310,6 +310,16 @@ class RaftApi:
             raise RaftError(st, self._p + "fsm_records_wait", f"{batch.n_dropped} records dropped")
         return recs, batch
 
+    def fsm_responses(self) -> Tuple[List[abi.FsmRecord], abi.FsmBatch]:
+        """jr_fsm_responses (F_CLIENT_RESPONSES): the ClientResponse runs of the batch most recently taken (by
+        fsm_records, drain_fsm, discard_fsm or a capturing step), copied out of the engine's pinned buffer.  Runs the
+        engine could not produce are counted in batch.n_dropped (the call's JR_E_CAPACITY) and are not an error here."""
+        ptr, batch = C.POINTER(abi.FsmRecord)(), abi.FsmBatch()
+        st = self._fn("fsm_responses")(self._h, C.byref(ptr), C.byref(batch))
+        if st != abi.E_CAPACITY:
+            self._check(st, "fsm_responses")
+        return [abi.FsmRecord.from_buffer_copy(ptr[i]) for i in range(batch.n_records)], batch
+
     def fsm_expand(self, records: Sequence[abi.FsmRecord]) -> List[abi.FsmInstr]:
         """jr_fsm_expand (pure host code of the engine library): records -> Instructions in jr_step order."""
         return expand_records(self._lib, records, self.n_groups, self.n_replicas)
@@ -550,6 +560,7 @@ def _bind(lib: C.CDLL, p: str):
         "leader_table": [vp, C.POINTER(abi.LeaderEntry)],
         "fsm_records_async": [vp],
         "fsm_records_wait": [vp, C.POINTER(C.POINTER(abi.FsmRecord)), C.POINTER(abi.FsmBatch)],
+        "fsm_responses": [vp, C.POINTER(C.POINTER(abi.FsmRecord)), C.POINTER(abi.FsmBatch)],
         "query_many": [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(abi.ReplicaState)],
         "chain_read_many": [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32),
                             C.c_size_t, C.POINTER(abi.Block), C.POINTER(C.c_uint8)],
@@ -603,6 +614,17 @@ def expand_records(lib: C.CDLL, records: Sequence[abi.FsmRecord], n_groups: int,
         if st != abi.OK:
             raise RaftError(st, "jr_fsm_expand")
     return [out[i] for i in range(need.value)]
+
+
+def expand_responses(runs: Sequence[abi.FsmRecord]) -> List[Tuple[int, int, Address, int, int]]:
+    """JR_FSMR_RESPONSE runs (as fsm_responses returns them) -> one (group, node, to, request token, block id) per
+    ClientResponse, group-major, node ascending, in each replica's apply order (the order fsm.rs:66-76 sends them)."""
+    out = []
+    for rc in sorted(runs, key=lambda rc: (rc.group, rc.node)):   # stable: FIFO per replica is kept
+        to = Address(rc.addr >> 16, rc.addr & 0xFFFF)
+        for i in range(rc.count):
+            out.append((rc.group, rc.node, to, (rc.tok0 + i * rc.stride) & 0xFFFFFFFFFFFFFFFF, rc.id0 + i))
+    return out
 
 
 def _open_engine_library(path: str) -> C.CDLL:

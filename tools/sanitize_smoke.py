@@ -68,3 +68,24 @@ for rnd in range(3):
     e.fsm_records()
 print("one-lane fold", e.fold_count(), e.state_digest(), e.fault_count())
 print("round-2 sanitize workload done")
+
+# client responses: fsm::Driver's map on the device (fsm_respond_kernel), fed by every drain path
+for fl in (0, abi.F_NO_SYMMETRIC_FOLD):
+    e = RaftEngine.create(64, 5, seed=7, flags=abi.F_CAPTURE_FSM | abi.F_CLIENT_RESPONSES | fl, chain_capacity=64, fsm_units=32)
+    e.step(0, flags=0, inject=bootstrap(64, 5))
+    e.set_auto_truncate(4)
+    e.run(100, 100, 10, 0)
+    e.leader_table()
+    answered = 0
+    for rnd in range(4):
+        e.run_token_runs(1100 + 2000 * rnd, 100, 20, [((rnd + 1) << 40 | (g + 1), 1 << 20) for g in range(64)])
+        if rnd % 2:
+            e.fsm_records()
+        else:
+            e.discard_fsm()
+        answered += e.fsm_responses()[1].n_instructions
+    e.node_restart_many(9100, [(g, 1, None, 0, None) for g in range(0, 64, 3)])
+    e.run(9100, 100, 8, 0)
+    e.drain_fsm()
+    print("client responses", fl, answered, e.fsm_responses()[1].n_instructions)
+print("client-response sanitize workload done")
