@@ -1118,6 +1118,7 @@ struct jr_engine {
   // symmetric-group fold
   uint8_t* symdone = nullptr;   // device, Gp entries
   uint8_t* symblk = nullptr;    // device, Gp / 32 entries
+  uint32_t* symrec = nullptr;   // device, sym_record_words(R) x Gp: sym_check_kernel's entry records (transient, see sym_fold.cuh)
   bool auto_trunc = false;      // jr_set_auto_truncate
   uint32_t auto_trunc_margin = 0;
   int no_fold = 0;              // JR_NO_FOLD=1 (A/B, tests)
@@ -1221,11 +1222,14 @@ static jr_status launch_step(jr_engine* e, const StepParams& p_in) {
 template <int R>
 static void launch_sym_r(jr_engine* e, const StepParams& p) {
   if constexpr (R >= 2) {
+    // the entry checks, then the fold that consumes their records: nothing may run between the two
+    JR_LAUNCH(sym_check_kernel<R>, (e->d.Gp + SYM_CHECK_THREADS - 1) / SYM_CHECK_THREADS, SYM_CHECK_THREADS, e->stream, e->d, p,
+              e->symrec);
     if (e->sym_one_lane)
-      JR_LAUNCH(sym_kernel<R>, (e->d.Gp + SYM_LANES - 1) / SYM_LANES, SYM_LANES, e->stream, e->d, p, e->symdone);
+      JR_LAUNCH(sym_kernel<R>, (e->d.Gp + SYM_LANES - 1) / SYM_LANES, SYM_LANES, e->stream, e->d, p, e->symdone, e->symrec);
     else
       JR_LAUNCH_SMEM(sym2_kernel<R>, (e->d.Gp + SYM2_GROUPS - 1) / SYM2_GROUPS, 2 * SYM2_GROUPS,
-                     (size_t)SYM2_UNITS * SYM2_GROUPS * sizeof(uint4), e->stream, e->d, p, e->symdone, e->symblk);
+                     (size_t)SYM2_UNITS * SYM2_GROUPS * sizeof(uint4), e->stream, e->d, p, e->symdone, e->symblk, e->symrec);
   }
 }
 
@@ -1386,6 +1390,7 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
   A(d.tb, d.Gp);
   A(e->symdone, d.Gp);
   A(e->symblk, d.Gp / GROUPS_PER_CTA);
+  A(e->symrec, (size_t)sym_record_words(d.R) * d.Gp);
   if (d.flags & JR_F_CAPTURE_FSM) {
     const size_t reps = (size_t)cfg->n_groups * cfg->n_replicas;   // default: 2 per replica, but never less than a small engine's whole FIFO space
     const size_t want = cfg->fsm_host_records ? cfg->fsm_host_records

@@ -13,9 +13,10 @@
 // barrier per tick; sym_kernel runs both in one lane with the mail in registers.
 //
 // Exactness contract:
-//   * Both FIRST CHECK that a group is symmetric, that its followers' tables agree over every id the launch can read,
-//     and that its mail in flight has the canonical shapes (sym_enter); every other group is left to step_kernel
-//     untouched.
+//   * sym_check_kernel, launched right before either of them with nothing in between, FIRST CHECKS that a group is
+//     symmetric, that its followers' tables agree over every id the launch can read, and that its mail in flight has the
+//     canonical shapes (sym_enter), on the planes the fold is about to read; every other group is left to step_kernel
+//     untouched.  The fold takes the verdict and its starting state from the entry record the check leaves behind.
 //   * If anything outside the canonical evolution would happen during the launch (a fault, an election timer that
 //     could fire, a HeartbeatResponse{has_committed: false}, a read below the compared rows, ...) the lane ABORTS (in
 //     sym2_kernel: tells the other lane through the mail, and both check the other's last mail after the last
@@ -105,11 +106,12 @@ enum : uint32_t {
   SP_HB = 7,           // followers: Heartbeat and its apply range
   SP_SCAN = 8,         // followers: the replicate() scan over the leader's rows (fetch_sent)
   SP_EXTEND = 9,       // followers: follower_extend, the R-1 row stores
-  SP_ENTER = 10, SP_FILL = 11, SP_LEAVE = 12, SP_TRUNC = 13,   // once per launch: sym_enter (with its barriers), cache fill +
+  SP_ENTER = 10, SP_FILL = 11, SP_LEAVE = 12, SP_TRUNC = 13,   // once per launch: the entry record load, cache fill +
                                                                // encoder init, sym_leave_*, the fused truncation
 };
 
-template <int R, bool SPLIT = false>
+// CHECK: the group as sym_check_kernel sees it -- no row caches, every table read goes to global memory.
+template <int R, bool SPLIT = false, bool CHECK = false>
 struct SymGroup {
   static constexpr uint32_t STRIDE = SPLIT ? SYM2_GROUPS : SYM_LANES;   // columns of the CTA's per-group shared memory
   const Dev& d;
@@ -163,6 +165,7 @@ struct SymGroup {
   // r is the leader (its own table) or F0 (the followers' table)
   __device__ __forceinline__ void fetch(uint32_t r, uint32_t bid, uint32_t& next, uint64_t& tok) {
     if (!in_window(bid)) { next = ABSENT; tok = 0; return; }
+    if (CHECK) { next = d.cnext[row(r, bid)]; tok = d.ctok[row(r, bid)]; return; }
     const uint4 e = slot(r, bid);
     if (e.x == bid) { next = e.y; tok = (uint64_t)e.z | ((uint64_t)e.w << 32); return; }
     next = __ldcg(d.cnext + row(r, bid));   // rows written earlier in this launch by this lane: read them at L2
@@ -534,9 +537,9 @@ struct SymGroup {
   }
 };
 
-// ---- entry: is the group symmetric, is its mail canonical? ---------------------------------------------------------
-template <int R, bool SPLIT>
-__device__ __forceinline__ bool sym_enter(SymGroup<R, SPLIT>& s, SymMail& m, const StepParams& p, int prv) {
+// ---- entry: is the group symmetric, is its mail canonical? (run by sym_check_kernel, below) ---------------------------
+template <int R>
+__device__ __forceinline__ bool sym_enter(SymGroup<R, false, true>& s, SymMail& m, const StepParams& p, int prv) {
   const Dev& d = s.d;
   if (s.g >= d.G) return false;
   // roles: one live leader, R-1 live followers of that leader
@@ -738,17 +741,140 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, SPLIT>& s, SymMail& m, con
   return true;
 }
 
+// ---- entry record ------------------------------------------------------------------------------------------------------
+// sym_check_kernel runs sym_enter for every group, one thread each, right before the fold kernel, and leaves its verdict
+// and everything the fold takes from the state planes in the entry record: [word][group] planes of 32-bit words (Gp
+// groups per plane), so that every warp's loads and stores are coalesced.  The fold kernels load the words of their
+// side in one round instead of walking sym_enter's chain of dependent loads with a quarter of the warps in flight.
+// Only sym_leave_* writes these planes of a folded group between the two kernels, so the words carried to the exit are
+// the ones it would read there.  Transient: rewritten by every pre-pass, not part of a checkpoint.
+//   SR_FLAGS      ok | L << 1 | ckey << 4 | fckey << 5 | mode_self << 6 | mode_f << 7 | mail in flight: hb << 8 | ae << 9 |
+//                 ae_nb << 10 | hbr << 13 | hbr_has << 14 | ar << 15 | share << 16   (only this word when !ok)
+//   leader        head, commit, idgen, maxkey, ph_self, ph_f, hbtime, hb_commit, ae_id[5], fc[L] (0 without capture)
+//   followers     fhead, fcommit, fmaxkey, flo, hbr_commit, ar_head
+//   exit          term; the upper half of every replica's P2 .w with ckey cleared (the lower half is its role: faults
+//                 exclude a group), two per word; per follower, in replica order: P1 .w (RNG draws), then P2 .z
+enum : uint32_t {
+  SR_FLAGS = 0, SR_TBASE,
+  SR_HEAD, SR_COMMIT, SR_IDGEN, SR_MAXKEY, SR_PH_SELF, SR_PH_F, SR_HBTIME, SR_HB_COMMIT = SR_HBTIME + 2,
+  SR_AE_ID, SR_FC_L = SR_AE_ID + JR_MAX_AE_BLOCKS,
+  SR_FHEAD = SR_FC_L + 2, SR_FCOMMIT, SR_FMAXKEY, SR_FLO, SR_HBR_COMMIT, SR_AR_HEAD,
+  SR_TERM, SR_P2W = SR_TERM + 2,
+};
+__host__ __device__ constexpr uint32_t sr_draws(uint32_t R) { return SR_P2W + (R + 1) / 2; }
+__host__ __device__ constexpr uint32_t sr_idgen(uint32_t R) { return sr_draws(R) + R - 1; }
+__host__ __device__ constexpr uint32_t sym_record_words(uint32_t R) { return sr_idgen(R) + R - 1; }
+
+// One thread per group, 128-thread CTAs.  The checks are chains of dependent loads, so what makes them go faster is the
+// number of chains in flight -- but sym_enter wants ~126 registers, and spills cost more than warps gain: 5 CTAs per SM
+// (96 registers, no spills, 20 warps) ran the pre-pass in 45 us on the H100 at the headline shape, 8 CTAs (64
+// registers, 100 B of spill stores) in 49 us, 12 CTAs (40 registers, 492 B) in 55 us.  (A/B builds override it.)
+#ifndef JR_SYM_CHECK_MINCTAS
+#define JR_SYM_CHECK_MINCTAS 5
+#endif
+constexpr uint32_t SYM_CHECK_THREADS = 128;
+template <int R>
+__global__ void __launch_bounds__(SYM_CHECK_THREADS, JR_SYM_CHECK_MINCTAS) sym_check_kernel(const Dev d, const StepParams p, uint32_t* rec) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= d.Gp) return;
+  const size_t n = d.Gp;
+  uint32_t* w = rec + g;
+  SymGroup<R, false, true> s(d, g);
+  SymMail m;
+  if (!sym_enter(s, m, p, 1 - p.cur)) { w[SR_FLAGS * n] = 0u; return; }
+  const uint32_t L = s.L;
+  const bool cap = (d.flags & JR_F_CAPTURE_FSM) != 0;
+  bool share = cap;                                          // the followers' Instruction FIFOs are all empty
+  uint32_t hw[(R + 1) / 2];
+#pragma unroll
+  for (int k = 0; k < (R + 1) / 2; ++k) hw[k] = 0;
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const uint4 c = d.p2[s.rg(r)];
+    hw[r / 2] |= ((c.w >> 16) & ~(1u << 12)) << (16 * (r & 1));
+    if ((uint32_t)r == L) continue;
+    const uint32_t k = (uint32_t)r - ((uint32_t)r > L ? 1u : 0u);
+    const uint2 fc = d.fc[s.rg(r)];
+    if (fc.x | fc.y) share = false;
+    w[(sr_draws(R) + k) * n] = d.p1[s.rg(r)].w;
+    w[(sr_idgen(R) + k) * n] = c.z;
+  }
+  const uint2 fcl = cap ? d.fc[s.rg(L)] : make_uint2(0u, 0u);
+  w[SR_FLAGS * n] = 1u | (L << 1) | (s.ckey << 4) | (s.fckey << 5) | (s.mode_self << 6) | (s.mode_f << 7) | (m.hb << 8) |
+                    (m.ae << 9) | (m.ae_nb << 10) | (m.hbr << 13) | (m.hbr_has << 14) | (m.ar << 15) | ((share ? 1u : 0u) << 16);
+  w[SR_TBASE * n] = s.tbase;
+  w[SR_HEAD * n] = s.head; w[SR_COMMIT * n] = s.commit; w[SR_IDGEN * n] = s.idgen; w[SR_MAXKEY * n] = s.maxkey;
+  w[SR_PH_SELF * n] = s.ph_self; w[SR_PH_F * n] = s.ph_f;
+  w[SR_HBTIME * n] = (uint32_t)s.hbtime; w[(SR_HBTIME + 1) * n] = (uint32_t)(s.hbtime >> 32);
+  w[SR_HB_COMMIT * n] = m.hb_commit;
+#pragma unroll
+  for (uint32_t k = 0; k < JR_MAX_AE_BLOCKS; ++k) w[(SR_AE_ID + k) * n] = m.ae_id[k];
+  w[SR_FC_L * n] = fcl.x; w[(SR_FC_L + 1) * n] = fcl.y;
+  w[SR_FHEAD * n] = s.fhead; w[SR_FCOMMIT * n] = s.fcommit; w[SR_FMAXKEY * n] = s.fmaxkey; w[SR_FLO * n] = s.flo;
+  w[SR_HBR_COMMIT * n] = m.hbr_commit; w[SR_AR_HEAD * n] = m.ar_head;
+  w[SR_TERM * n] = (uint32_t)s.term; w[(SR_TERM + 1) * n] = (uint32_t)(s.term >> 32);
+#pragma unroll
+  for (int k = 0; k < (R + 1) / 2; ++k) w[(SR_P2W + k) * n] = hw[k];
+}
+
+// The entry record of group s.g (< Gp), one round of loads: LEAD the leader's side (and fc = its FSM counters), FOLLOW
+// the followers' side.  false: the group does not fold.
+template <bool LEAD, bool FOLLOW, int R, bool SPLIT>
+__device__ __forceinline__ bool sym_load(SymGroup<R, SPLIT>& s, SymMail& m, const uint32_t* rec, uint2& fc) {
+  const uint32_t* w = rec + s.g;
+  const size_t n = s.d.Gp;
+  const uint32_t f = __ldg(w + SR_FLAGS * n);
+  uint32_t v[SR_TERM];
+  if (LEAD) {
+#pragma unroll
+    for (uint32_t k = SR_TBASE; k < SR_FHEAD; ++k) v[k] = __ldg(w + k * n);
+  }
+  if (FOLLOW) {
+#pragma unroll
+    for (uint32_t k = SR_FHEAD; k < SR_TERM; ++k) v[k] = __ldg(w + k * n);
+    if (!LEAD) v[SR_TBASE] = __ldg(w + SR_TBASE * n);
+  }
+  if (!(f & 1u)) return false;
+  s.L = (f >> 1) & 7u;
+  s.F0 = s.L == 0 ? 1u : 0u;
+  s.tbase = v[SR_TBASE];
+  m = SymMail{};
+  if (LEAD) {
+    s.ckey = (f >> 4) & 1u; s.mode_self = (f >> 6) & 1u; s.mode_f = (f >> 7) & 1u;
+    s.head = v[SR_HEAD]; s.commit = v[SR_COMMIT]; s.idgen = v[SR_IDGEN]; s.maxkey = v[SR_MAXKEY];
+    s.ph_self = v[SR_PH_SELF]; s.ph_f = v[SR_PH_F];
+    s.hbtime = (uint64_t)v[SR_HBTIME] | ((uint64_t)v[SR_HBTIME + 1] << 32);
+    m.hb = (f >> 8) & 1u; m.ae = (f >> 9) & 1u; m.ae_nb = (f >> 10) & 7u;
+    m.hb_commit = v[SR_HB_COMMIT];
+#pragma unroll
+    for (uint32_t k = 0; k < JR_MAX_AE_BLOCKS; ++k) m.ae_id[k] = v[SR_AE_ID + k];
+    fc = make_uint2(v[SR_FC_L], v[SR_FC_L + 1]);
+  }
+  if (FOLLOW) {
+    s.fckey = (f >> 5) & 1u;
+    s.share = (f >> 16) & 1u;
+    s.fhead = v[SR_FHEAD]; s.fcommit = v[SR_FCOMMIT]; s.fmaxkey = v[SR_FMAXKEY]; s.flo = v[SR_FLO];
+    m.hbr = (f >> 13) & 1u; m.hbr_has = (f >> 14) & 1u; m.ar = (f >> 15) & 1u;
+    m.hbr_commit = v[SR_HBR_COMMIT]; m.ar_head = v[SR_AR_HEAD];
+  }
+  return true;
+}
+
 // ---- exit: write everything step_kernel would have left behind -------------------------------------------------------
 template <int R, bool SPLIT>
-__device__ __forceinline__ void sym_leave_leader(SymGroup<R, SPLIT>& s, const SymMail& last, int cur_last) {
+__device__ __forceinline__ void sym_leave_leader(SymGroup<R, SPLIT>& s, const SymMail& last, int cur_last, const uint32_t* rec) {
   const Dev& d = s.d;
   const uint32_t L = s.L;
   {  // leader: P2, P3, progress planes, max key (P0 / P1 are untouched by a steady leader)
     const size_t i = s.rg(L);
+    const uint32_t* w = rec + s.g;
+    const size_t n = d.Gp;
+    const uint32_t t0 = __ldg(w + SR_TERM * n), t1 = __ldg(w + (SR_TERM + 1) * n), hw = __ldg(w + (SR_P2W + L / 2) * n);
+    s.term = (uint64_t)t0 | ((uint64_t)t1 << 32);
     uint32_t prmask = 0;
 #pragma unroll
     for (int r = 0; r < R; ++r) prmask |= (((uint32_t)r == L ? s.mode_self : s.mode_f) & 1u) << r;
-    const uint32_t keep = d.p2[i].w & ~((255u << 16) | (1u << 28));
+    const uint32_t keep = (JR_ROLE_LEADER | (((hw >> (16 * (L & 1u))) & 0xffffu) << 16)) & ~((255u << 16) | (1u << 28));
     d.p2[i] = make_uint4(s.head, s.commit, s.idgen, keep | (prmask << 16) | (s.ckey << 28));
     d.p3[i] = make_uint4((uint32_t)s.hbtime, (uint32_t)(s.hbtime >> 32), 0u, 0u);
 #pragma unroll
@@ -792,25 +918,39 @@ __device__ __forceinline__ void sym_leave_leader(SymGroup<R, SPLIT>& s, const Sy
 }
 
 template <int R, bool SPLIT>
-__device__ __forceinline__ void sym_leave_followers(SymGroup<R, SPLIT>& s, const SymMail& last, int cur_last) {
+__device__ __forceinline__ void sym_leave_followers(SymGroup<R, SPLIT>& s, const SymMail& last, int cur_last, const uint32_t* rec) {
   const Dev& d = s.d;
   const uint32_t L = s.L;
   // The followers emitted the same Instructions.  If none of them has anything pending since the last drain, ONE set of
   // records (in the lowest follower's FIFO, APPLY records carrying the mask of all followers) stands for all of them;
   // the others only advance their Instruction counters.  Otherwise every follower gets its own copy.
   const bool shared_records = s.share;
+  // the followers' P1 .w, P2 .z and upper half of P2 .w, as sym_check_kernel found them: independent loads first
+  const uint32_t* w = rec + s.g;
+  const size_t n = d.Gp;
+  const uint32_t t0 = __ldg(w + SR_TERM * n), t1 = __ldg(w + (SR_TERM + 1) * n);
+  uint32_t hw[(R + 1) / 2], draws0[R], idgen[R];
+#pragma unroll
+  for (int k = 0; k < (R + 1) / 2; ++k) hw[k] = __ldg(w + (SR_P2W + k) * n);
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    if ((uint32_t)r == L) continue;
+    const uint32_t k = (uint32_t)r - ((uint32_t)r > L ? 1u : 0u);
+    draws0[r] = __ldg(w + (sr_draws(R) + k) * n);
+    idgen[r] = __ldg(w + (sr_idgen(R) + k) * n);
+  }
+  s.term = (uint64_t)t0 | ((uint64_t)t1 << 32);
 #pragma unroll
   for (int r = 0; r < R; ++r) {   // followers: P1 (timer, RNG), P2, max key, outbox
     if ((uint32_t)r == L) continue;
     const size_t i = s.rg(r);
     if (s.n_hb) {                  // follower.rs:103-113 per heartbeat: only the last draw is visible
-      const uint4 b = d.p1[i];
-      const uint32_t draws = b.w + s.n_hb;
+      const uint32_t draws = draws0[r] + s.n_hb;
       d.p1[i] = make_uint4((uint32_t)s.last_hb, (uint32_t)(s.last_hb >> 32),
                            election_timeout_draw(d.seed, d.goff + s.g, r + 1, draws - 1, d.emin, d.emax), draws);
     }
-    const uint4 c = d.p2[i];
-    d.p2[i] = make_uint4(s.fhead, s.fcommit, c.z, (c.w & ~(1u << 28)) | (s.fckey << 28));
+    const uint32_t upper = (hw[r / 2] >> (16 * (r & 1))) & 0xffffu;
+    d.p2[i] = make_uint4(s.fhead, s.fcommit, idgen[r], (JR_ROLE_FOLLOWER | (upper << 16)) | (s.fckey << 28));
     d.mk[i] = s.fmaxkey;
     uint32_t u = 0;
     if (last.hbr)
@@ -830,7 +970,8 @@ __device__ __forceinline__ void sym_leave_followers(SymGroup<R, SPLIT>& s, const
 
 // One lane per group.  symdone[g] = 1: the whole launch of group g has been applied here; 0: step_kernel runs it.
 template <int R>
-__global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const Dev d, const StepParams p, uint8_t* symdone) {
+__global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const Dev d, const StepParams p, uint8_t* symdone,
+                                                                        const uint32_t* rec) {
   const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= d.Gp) return;
   SymGroup<R> s(d, g);
@@ -845,18 +986,12 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
   s.rows = lane_smem + threadIdx.x;
   s.enc = lane_smem + 2 * SYM_ROWS * SYM_LANES + threadIdx.x;
   s.cache_clear();
-  bool ok = sym_enter(s, a, p, 1 - p.cur);
+  uint2 fcl;
+  bool ok = sym_load<true, true>(s, a, rec, fcl);
   if (ok) {
     s.cache_fill(s.L, s.maxkey);
     s.cache_fill(s.F0, s.fmaxkey);
-    s.share = (d.flags & JR_F_CAPTURE_FSM) != 0;
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-      if ((uint32_t)r == s.L) continue;
-      const uint2 c = d.fc[s.rg(r)];
-      if (c.x | c.y) s.share = false;
-    }
-    s.enc_init_leader((d.flags & JR_F_CAPTURE_FSM) ? d.fc[s.rg(s.L)] : make_uint2(0u, 0u));
+    s.enc_init_leader(fcl);
     s.enc_init_followers();
     const jr_proposal* props = p.proposals;
     s.now = p.now;
@@ -887,15 +1022,15 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
     ok = !s.abort;
     if (ok) {
       const int cur_last = p.cur ^ (int)((p.n_ticks - 1) & 1u);
-      sym_leave_leader(s, a, cur_last);
-      sym_leave_followers(s, a, cur_last);
+      sym_leave_leader(s, a, cur_last, rec);
+      sym_leave_followers(s, a, cur_last, rec);
     }
   }
   symdone[g] = ok ? 1 : 0;
 }
 
-// Two lanes per group (see SYM2_GROUPS above).  Both lanes run sym_enter on the same, still untouched planes and reach
-// the same verdict; afterwards each keeps to its side: the leader lane owns the leader's table cache, encoder state,
+// Two lanes per group (see SYM2_GROUPS above).  Both lanes take the same verdict from the group's entry record, each
+// loading the words of its side; afterwards each keeps to its side: the leader lane owns the leader's table cache, encoder state,
 // planes and outbox, the follower lane those of the followers.  Either side may abort: it says so in its mail, the
 // other side sees it one barrier later, and after the last barrier both check the other's final mail, so a group is
 // either left (by both) or not at all.
@@ -909,7 +1044,8 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
 #define JR_SYM2_ROLES 3   // (register-need experiments: 1 = leader code only, 2 = follower code only)
 #endif
 template <int R>
-__global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(const Dev d, const StepParams p, uint8_t* symdone, uint8_t* symblk) {
+__global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(const Dev d, const StepParams p, uint8_t* symdone, uint8_t* symblk,
+                                                                                      const uint32_t* rec) {
   JR_DYN_SMEM(uint4, smem);
   // One __syncthreads() per tick for both warp pairs of the CTA.  (A named barrier per pair -- `bar.sync 0/1, 64`, the
   // pairs never need each other -- was slower; with a register operand for the id ptxas charges the CTA
@@ -919,7 +1055,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   const bool lead = ((w ^ blockIdx.x) & 1u) == 0;          // roles alternate from CTA to CTA: no SM sub-partition gets leaders only
   const uint32_t gi = (w >> 1) * 32u + lane;               // group within the CTA
-  const uint32_t g = blockIdx.x * S + gi;                  // (g >= Gp: sym_enter says no; the lane only keeps the barriers company)
+  const uint32_t g = blockIdx.x * S + gi;                  // (g >= Gp: no record; the lane only keeps the barriers company)
   SymGroup<R, true> s(d, g);
   s.abort = false;
   s.lcnt = s.fcnt = 0;
@@ -939,28 +1075,20 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.cache_clear(lead ? 0u : SYM_ROWS, SYM_ROWS);
   const uint32_t blk = g / GROUPS_PER_CTA;                  // step_kernel's 32-group block of this warp pair
   if (lead && lane == 0 && g < d.Gp) symblk[blk] = 1;      // (cleared below by any lane whose group is not folded)
-  pair_sync();
   SymMail a;
-  bool dead = !sym_enter(s, a, p, 1 - p.cur);
-  pair_sync();                                         // the other lane's sym_enter may still be reading this lane's (empty) cache
+  uint2 fcl;
+  bool dead = g >= d.Gp || !(lead ? sym_load<true, false>(s, a, rec, fcl) : sym_load<false, true>(s, a, rec, fcl));
   s.phase(SP_FILL);
   if (!dead) {
     if (lead) {
       s.cache_fill(s.L, s.maxkey);
-      s.enc_init_leader((d.flags & JR_F_CAPTURE_FSM) ? d.fc[s.rg(s.L)] : make_uint2(0u, 0u));
+      s.enc_init_leader(fcl);
       // the mail in flight, where tick 0 looks for it
       mail[2 * S] = make_uint4(a.hb | (a.ae << 1) | (a.ae_nb << 4) | SYM2_IDS, a.hb_commit, s.maxkey, a.ae_id[0]);
       mail[3 * S] = make_uint4(a.ae_id[1], a.ae_id[2], a.ae_id[3], a.ae_id[4]);
     } else {
       s.cache_fill(s.F0, s.fmaxkey);
       s.enc_init_followers();
-      s.share = (d.flags & JR_F_CAPTURE_FSM) != 0;
-#pragma unroll
-      for (int r = 0; r < R; ++r) {
-        if ((uint32_t)r == s.L) continue;
-        const uint2 c = d.fc[s.rg(r)];
-        if (c.x | c.y) s.share = false;
-      }
       mail[5 * S] = make_uint4(a.hbr | (a.hbr_has << 1) | (a.ar << 2), a.hbr_commit, a.ar_head, 0u);
     }
   }
@@ -1040,11 +1168,11 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
       last.hb = la.x & 1u; last.ae = (la.x >> 1) & 1u;
       last.hb_commit = la.y;
       if (last.ae) s.replicate(s.ph_f, s.mode_f, s.maxkey, last);   // what the last tick sent: the outbox it leaves behind
-      sym_leave_leader(s, last, cur_last);
+      sym_leave_leader(s, last, cur_last, rec);
     } else {
       last.hbr = lc.x & 1u; last.hbr_has = (lc.x >> 1) & 1u; last.ar = (lc.x >> 2) & 1u;
       last.hbr_commit = lc.y; last.ar_head = lc.z;
-      sym_leave_followers(s, last, cur_last);
+      sym_leave_followers(s, last, cur_last, rec);
     }
   }
   s.phase(SP_TRUNC);

@@ -2,7 +2,7 @@
 """Where one bench step's device time goes: CUDA events between the three calls of a step (fused run, truncate, drain)
 on the engine's stream, for the headline workload and its variants.  Diagnostic; bench.py holds the reported numbers.
 
-usage: step_breakdown.py [steps]"""
+usage: step_breakdown.py [steps] [--kernels]"""
 import argparse
 import ctypes as C
 import os
@@ -65,16 +65,51 @@ def measure(bn, label, G, R, steps, capture=True, flush=True, **kw):
     torch.cuda.empty_cache()
 
 
+def kernel_times(bn, G, R, steps):
+    """Device time per step of every kernel of the headline step (fused run with its pre-pass, drain), from torch.profiler
+    in a run of its own: CUDA events between the calls cannot split the fused run into its kernels."""
+    from torch.profiler import ProfilerActivity, profile
+    torch = bn.torch
+    eng = bn.steady_engine(G, R, abi.F_CAPTURE_FSM, auto_truncate=True)
+    S = bench.TICKS_PER_STEP
+    now = bench.DT_MS * 17
+
+    def step():
+        nonlocal now
+        bn.flush.fill_(1)
+        eng.run(now, bench.DT_MS, S, 1)
+        eng.discard_fsm(strict=False)
+        now += bench.DT_MS * S
+
+    for _ in range(5):
+        step()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            step()
+        torch.cuda.synchronize()
+    rows = [(k.self_device_time_total / steps, k.count / steps, k.key) for k in prof.key_averages() if k.self_device_time_total > 0]
+    print(f"kernels of the headline step ({G} groups x {R} replicas, {steps} steps, L2 flushed), us per step:", flush=True)
+    for us, n, name in sorted(rows, reverse=True):
+        print(f"  {us:9.1f}  x{n:4.1f}  {name[:100]}", flush=True)
+    del eng
+    torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("steps", nargs="?", type=int, default=60)
     ap.add_argument("--only", type=int, default=99, help="run only the first N variants")
     ap.add_argument("--explicit-truncate", action="store_true", help="jr_truncate as its own call (the pre-fusion shape)")
+    ap.add_argument("--kernels", action="store_true", help="instead: each kernel's device time in the headline step (torch.profiler)")
     a = ap.parse_args()
     global EXPLICIT_TRUNCATE
     EXPLICIT_TRUNCATE = a.explicit_truncate
     bn = bench.Bench(argparse.Namespace())
     G, R = bench.GROUPS_PER_GPU, bench.REPLICAS
+    if a.kernels:
+        kernel_times(bn, G, R, a.steps)
+        return
     variants = [("headline", G, {}), ("headline, no capture", G, {"capture": False}), ("scattered leaders", G, {"scattered": True}),
                 ("headline, warm L2 (no flush)", G, {"flush": False}), ("heartbeat every tick", G, {"heartbeat_ms": 99}),
                 ("131,072 groups", 2 * G, {}), ("headline, fold off (step_kernel)", G, {"_nofold": True}),

@@ -23,7 +23,7 @@ from josefine_b200 import abi, RaftEngine  # noqa: E402
 TICK = {0: "mail read (+ proposal)", 1: "AppendResponse (leader_commit loop)", 2: "client_request", 3: "NOTIFY encoder pushes",
         4: "APPLY encoder pushes", 5: "heartbeat / mail write", 7: "heartbeat + apply range", 8: "replicate scan (fetch_sent)",
         9: "follower_extend (row stores)", 6: "barrier wait"}
-LAUNCH = {10: "sym_enter", 11: "cache fill + encoder init", 12: "sym_leave", 13: "fused truncation"}
+LAUNCH = {10: "entry record load", 11: "cache fill + encoder init", 12: "sym_leave", 13: "fused truncation"}
 LEADER, FOLLOWER = 2, 0
 
 
