@@ -32,6 +32,8 @@
  *   jr_chain_export_many <- the sled trees of many nodes: the block records and the "commit" key
  *                         Chain::new / append / extend / commit writing sled  src/raft/chain.rs:119-123,160-205
  *   jr_query_many / jr_chain_read_many <- the same pub fields, for many replicas in one call
+ *   jr_verify_groups   <- no reference API: a check of Raft's own invariants over every replica's committed chain
+ *                         (an operator's replica verification tool)
  *   jr_engine_save / jr_engine_restore <- checkpoint of the whole engine (no reference API: sled persistence of
  *                         every node at once, chain.rs:119-123,198, plus the volatile State the reference loses)
  *   jr_truncate        <- no reference API (deviation D7)
@@ -572,6 +574,73 @@ jr_status jr_chain_export_many(jr_engine* e, const uint32_t* groups, const uint3
  */
 jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted_chain* chains, size_t n,
                                const jr_block* blocks, size_t n_blocks);
+
+/*
+ * ---- replica verification ----------------------------------------------------------------------------------------
+ * Checks on the device that the replicas of each group hold the same committed chain.  The reference never compares
+ * what its replicas committed: a follower commits an id it merely holds (follower.rs:200-204, chain.rs:195-205) and
+ * Chain::extend overwrites whatever sat under an id (chain.rs:178-192).  Normative, for group g with floor F (D7) and
+ * window W = chain_capacity:
+ *   Checked replicas are alive and unfaulted; silenced and faulted replicas are counted as skipped.  present(n, x) means
+ *   F <= x < F + W and replica n holds block x; row_n(x) = (next, token).  Per checked replica n with commit c_n, in order:
+ *     JR_VERIFY_BELOW_FLOOR    c_n < F: the committed chain has left the window and cannot be checked (not a
+ *                              violation: a replica revived after the floor passed it).  id = c_n.
+ *     JR_VERIFY_COMMIT_ABSENT  !present(n, c_n).  id = c_n.
+ *     JR_VERIFY_CHAIN_BROKEN   the committed chain chain(n) = c_n, next(c_n), ... -- which stops at the first id below F
+ *                              and after the genesis block 0 -> 0 -- reaches an id x >= F that is not present, or a
+ *                              block x other than genesis whose next is not below x (a cycle a forged extend can make).
+ *                              id = x.  A walk takes at most W steps.
+ *   The reference replica ref(g) is, among the checked replicas with an intact chain, the one with the largest commit;
+ *   ties go to the smallest node id.  Every other intact replica n is
+ *     JR_VERIFY_DIVERGED       if c_n is not on chain(ref) (id = c_n), or else if some x on chain(n) has
+ *                              row_n(x) != row_ref(x) (id = the highest such x);
+ *   otherwise it is OK and produces no finding.  Equivalently: the committed chain of every replica is a prefix of the
+ *   reference's, block for block, within the window.
+ *     JR_VERIFY_LEADER_CONFLICT two or more checked replicas of the group are Leader with the same current_term.  One
+ *                              finding per (group, term): node = 0, node_mask = those leaders, term = that term.
+ */
+enum {
+  JR_VERIFY_BELOW_FLOOR = 1,
+  JR_VERIFY_COMMIT_ABSENT = 2,
+  JR_VERIFY_CHAIN_BROKEN = 3,
+  JR_VERIFY_DIVERGED = 4,
+  JR_VERIFY_LEADER_CONFLICT = 5
+};
+
+typedef struct jr_verify_report {
+  uint64_t groups_checked;
+  uint64_t replicas_checked;    /* alive and unfaulted replicas of those groups */
+  uint64_t replicas_skipped;    /* silenced or faulted */
+  uint64_t below_floor;         /* findings per kind */
+  uint64_t commit_absent;
+  uint64_t chain_broken;
+  uint64_t diverged;
+  uint64_t leader_conflicts;
+} jr_verify_report;
+
+/* One finding.  32 bytes. */
+typedef struct jr_verify_finding {
+  uint32_t group;
+  uint8_t  kind;       /* JR_VERIFY_* */
+  uint8_t  node;       /* the replica (1..R); 0 for JR_VERIFY_LEADER_CONFLICT */
+  uint8_t  ref_node;   /* the group's reference replica; 0 if no checked replica has an intact chain */
+  uint8_t  node_mask;  /* bit (id-1): the conflicting leaders, or the replica itself */
+  uint64_t id;         /* the block id the finding names (see above); 0 for JR_VERIFY_LEADER_CONFLICT */
+  uint64_t term;       /* the conflict's term, or the replica's current_term */
+  uint64_t reserved;
+} jr_verify_finding;
+
+/*
+ * Verify groups[0 .. n_groups) (groups == NULL and n_groups == 0: every group).  Fills *report and *n_findings, and
+ * findings[0 .. *n_findings), sorted by (group, node): a group's leader conflicts come first, ordered by their lowest
+ * leader, then its replica findings.  OK replicas produce no finding; a group whose replicas all agree costs no copy but
+ * the report's.  JR_E_INVAL, engine untouched, for a group out of range or named twice.  findings == NULL or
+ * cap < *n_findings: report and *n_findings are filled, JR_E_CAPACITY.  Synchronous on the engine stream and read-only:
+ * the state digest, the checkpoint and every later result are those of an engine that never verified.  It may run while
+ * jr_fsm_records_async / jr_leader_table_async batches are outstanding.
+ */
+jr_status jr_verify_groups(jr_engine* e, const uint32_t* groups, size_t n_groups, jr_verify_report* report,
+                           jr_verify_finding* findings, size_t cap, size_t* n_findings);
 /* Checkpoint: everything the engine holds (state planes, block tables, mailboxes, FIFOs, routing, counters).
  * jr_engine_save_size -> bytes needed; restore needs an engine created with the same jr_config. */
 jr_status jr_engine_save_size(jr_engine* e, size_t* bytes);

@@ -189,6 +189,59 @@ extern "C" {
     #[allow(dead_code)]
     fn jr_node_restart_many(e: *mut c_void, now_ms: u64, chains: *const JrPersistedChain, n: usize, blocks: *const JrBlock,
                             n_blocks: usize) -> c_int;
+    #[allow(dead_code)]
+    fn jr_verify_groups(e: *mut c_void, groups: *const u32, n_groups: usize, report: *mut JrVerifyReport,
+                        findings: *mut JrVerifyFinding, cap: usize, n_findings: *mut usize) -> c_int;
+}
+
+/// jr_verify_report: what one jr_verify_groups call checked, and its findings per kind.
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct JrVerifyReport {
+    pub groups_checked: u64,
+    pub replicas_checked: u64,
+    pub replicas_skipped: u64, // silenced or faulted
+    pub below_floor: u64,
+    pub commit_absent: u64,
+    pub chain_broken: u64,
+    pub diverged: u64,
+    pub leader_conflicts: u64,
+}
+
+/// jr_verify_finding (32 B): kind 1 BELOW_FLOOR, 2 COMMIT_ABSENT, 3 CHAIN_BROKEN, 4 DIVERGED, 5 LEADER_CONFLICT (node 0).
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct JrVerifyFinding {
+    pub group: u32,
+    pub kind: u8,
+    pub node: u8,
+    pub ref_node: u8,
+    pub node_mask: u8,
+    pub id: u64,
+    pub term: u64,
+    pub reserved: u64,
+}
+
+/// Sketch: right after `restart_hosted_groups`, check that the reopened replicas hold the committed chain their groups
+/// agree on -- a stale, misplaced or corrupt tree shows up as a finding before the broker serves from it.  `groups` are
+/// the restarted groups (empty: every group).  Two calls when something is found: the first one sizes the buffer.
+#[allow(dead_code)]
+unsafe fn verify_restarted_groups(engine: *mut c_void, groups: &[u32]) -> Result<(JrVerifyReport, Vec<JrVerifyFinding>), c_int> {
+    let (ptr, n) = if groups.is_empty() { (std::ptr::null(), 0) } else { (groups.as_ptr(), groups.len()) };
+    let mut report = JrVerifyReport::default();
+    let mut need = 0usize;
+    match jr_verify_groups(engine, ptr, n, &mut report, std::ptr::null_mut(), 0, &mut need) {
+        0 => return Ok((report, Vec::new())),
+        4 => {} // JR_E_CAPACITY: `need` findings
+        st => return Err(st),
+    }
+    let mut findings = vec![JrVerifyFinding::default(); need];
+    let st = jr_verify_groups(engine, ptr, n, &mut report, findings.as_mut_ptr(), findings.len(), &mut need);
+    if st != 0 {
+        return Err(st);
+    }
+    findings.truncate(need);
+    Ok((report, findings))
 }
 
 /// One replica's persisted sled tree (chain.rs:99-104): blocks[first_block .. first_block + n_blocks] + the commit key.

@@ -177,11 +177,35 @@ class PersistedChain(C.Structure):
                 ("n_blocks", C.c_uint32), ("commit_key", C.c_uint32)]
 
 
+# jr_verify_groups finding kinds (normative rules in the header)
+VERIFY_BELOW_FLOOR, VERIFY_COMMIT_ABSENT, VERIFY_CHAIN_BROKEN, VERIFY_DIVERGED, VERIFY_LEADER_CONFLICT = 1, 2, 3, 4, 5
+VERIFY_KIND_NAMES = {1: "BELOW_FLOOR", 2: "COMMIT_ABSENT", 3: "CHAIN_BROKEN", 4: "DIVERGED", 5: "LEADER_CONFLICT"}
+
+
+class VerifyReport(C.Structure):
+    """jr_verify_report: what one jr_verify_groups call checked, and its findings per kind."""
+    _fields_ = [("groups_checked", C.c_uint64), ("replicas_checked", C.c_uint64), ("replicas_skipped", C.c_uint64),
+                ("below_floor", C.c_uint64), ("commit_absent", C.c_uint64), ("chain_broken", C.c_uint64),
+                ("diverged", C.c_uint64), ("leader_conflicts", C.c_uint64)]
+
+    def as_tuple(self) -> tuple:
+        return tuple(getattr(self, k) for k, _ in self._fields_)
+
+
+class VerifyFinding(C.Structure):
+    """jr_verify_finding: one replica that is not OK, or one (group, term) with two or more leaders (node 0)."""
+    _fields_ = [("group", C.c_uint32), ("kind", C.c_uint8), ("node", C.c_uint8), ("ref_node", C.c_uint8),
+                ("node_mask", C.c_uint8), ("id", C.c_uint64), ("term", C.c_uint64), ("reserved", C.c_uint64)]
+
+    def as_tuple(self) -> tuple:
+        return (self.group, self.kind, self.node, self.ref_node, self.node_mask, self.id, self.term)
+
+
 # sizes the header implies (checked in tests/test_abi.py against offsetof-free arithmetic)
 EXPECTED_SIZES = {
     "Config": 72, "Block": 24, "Msg": 64 + 24 * MAX_AE_BLOCKS, "FsmInstr": 16 + 24,
     "Proposal": 16, "TokenRun": 16, "LeaderEntry": 16, "FsmRecord": 32, "FsmBatch": 24 + 4 * (MAX_REPLICAS + 1) + 4,
-    "ReplicaState": 160, "PersistedChain": 32,
+    "ReplicaState": 160, "PersistedChain": 32, "VerifyReport": 64, "VerifyFinding": 32,
 }
 
 # every symbol include/josefine_raft_abi.h declares
@@ -191,7 +215,7 @@ ENGINE_SYMBOLS = [
     "jr_chain_read", "jr_state_digest", "jr_stream_digest", "jr_fault_count", "jr_fold_count", "jr_compact",
     "jr_set_alive", "jr_kill_leaders", "jr_leader_table_device", "jr_leader_table", "jr_leader_table_async", "jr_leader_table_wait",
     "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_responses", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
-    "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
+    "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_verify_groups", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
 ]
 
 

@@ -624,6 +624,195 @@ __global__ void restart_marks_rebase_kernel(const Dev d, uint4* rm) {
   if (i < (size_t)d.R * d.Gp && rm[i].z) rm[i] = make_uint4(0u, 0u, 1u, 0u);
 }
 
+// ---- replica verification (jr_verify_groups; the rules are normative in the ABI header) -------------------------------
+// Read-only.  Two passes of one thread per replica of the listed groups, thread t = (node - 1) * n + list index: threads
+// are group-consecutive, so a warp over groups that sit at the same ids (steady state) loads each table row coalesced.
+//   verify_walk_kernel   the replica's own committed chain -> vw[t] = {verdict, id}
+//   verify_judge_kernel  the group's reference from its R verdicts; an intact replica other than the reference walks its
+//                        chain against the reference's; leader conflicts; the report's counts -> vf[t]
+// Only when there is something to report: verify_count / scan / pack put the findings in (group, node) order.
+constexpr uint32_t VW_SKIP = 0, VW_INTACT = 7;   // walk verdicts besides JR_VERIFY_BELOW_FLOOR .. JR_VERIFY_CHAIN_BROKEN
+constexpr int VERIFY_COUNTS = 7;                 // jr_verify_report from replicas_checked on
+
+__device__ __forceinline__ uint32_t verify_group(const uint32_t* groups, uint32_t j) { return groups ? groups[j] : j; }
+
+__global__ void verify_walk_kernel(const Dev d, const uint32_t* groups, uint32_t n, uint2* vw) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (size_t)d.R * n) return;
+  const uint32_t r = (uint32_t)(t / n), g = verify_group(groups, (uint32_t)(t % n));
+  const size_t plane = (size_t)d.R * d.Gp, i = (size_t)r * d.Gp + g;
+  const uint32_t meta = d.p2[i].w, cm = d.p2[i].y, floor = d.tb[g];
+  uint2 v = make_uint2(VW_SKIP, 0u);
+  if (((meta >> 8) & 255u) == 0 && ((meta >> 27) & 1u) == 0) {
+    if (cm < floor) {
+      v = make_uint2(JR_VERIFY_BELOW_FLOOR, cm);
+    } else if (cm - floor >= d.cap || d.cnext[(size_t)(cm & d.capm) * plane + i] == ABSENT) {
+      v = make_uint2(JR_VERIFY_COMMIT_ABSENT, cm);
+    } else {
+      v = make_uint2(VW_INTACT, cm);
+      uint32_t x = cm;
+      for (uint32_t s = 0; s < d.cap; ++s) {   // ids fall strictly inside [floor, floor + cap): at most cap steps
+        const uint32_t nx = d.cnext[(size_t)(x & d.capm) * plane + i];
+        // absent (ABSENT is above every id) or a next that is not below its id, genesis 0 -> 0 excepted
+        if (nx >= x && (x | nx) != 0) { v = make_uint2(JR_VERIFY_CHAIN_BROKEN, x); break; }
+        if (x == 0 || nx < floor) break;
+        x = nx;
+      }
+    }
+  }
+  vw[t] = v;
+}
+
+// vf[t] = {kind | ref node << 8 | conflict mask << 16, id}: kind 0 = no replica finding; the conflict mask is set on the
+// lowest leader of a term two or more checked leaders share.  rep += this CTA's counts (one atomic per count and CTA).
+__global__ void verify_judge_kernel(const Dev d, const uint32_t* groups, uint32_t n, const uint2* vw, uint2* vf,
+                                    unsigned long long* rep) {
+  __shared__ unsigned long long s[VERIFY_COUNTS][32];
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  uint64_t cnt[VERIFY_COUNTS] = {0, 0, 0, 0, 0, 0, 0};   // checked, skipped, below floor, absent, broken, diverged, conflicts
+  if (t < (size_t)d.R * n) {
+    const uint32_t r = (uint32_t)(t / n), j = (uint32_t)(t % n), g = verify_group(groups, j);
+    const size_t plane = (size_t)d.R * d.Gp, i = (size_t)r * d.Gp + g;
+    uint32_t ref = 0, refc = 0;   // node id, commit
+    for (uint32_t k = 0; k < d.R; ++k) {
+      const uint2 w = vw[(size_t)k * n + j];
+      if (w.x == VW_INTACT && (ref == 0 || w.y > refc)) { ref = k + 1; refc = w.y; }
+    }
+    const uint2 mine = vw[t];
+    uint32_t kind = mine.x == VW_INTACT ? 0u : mine.x, id = mine.y, lc = 0;
+    if (mine.x == VW_INTACT && ref != r + 1) {
+      const size_t ir = (size_t)(ref - 1) * d.Gp + g;
+      const uint32_t cm = mine.y, floor = d.tb[g];
+      uint32_t y = refc;   // down the reference's chain to the first id <= c_n: c_n is on it iff that id is c_n
+      for (uint32_t s2 = 0; s2 < d.cap && y > cm; ++s2) y = d.cnext[(size_t)(y & d.capm) * plane + ir];
+      if (y != cm) {
+        kind = JR_VERIFY_DIVERGED;
+      } else {             // then both chains share every block down to the first row that differs
+        uint32_t x = cm;
+        for (uint32_t s2 = 0; s2 < d.cap; ++s2) {
+          const size_t row = (size_t)(x & d.capm) * plane;
+          const uint32_t nx = d.cnext[row + i];
+          if (nx != d.cnext[row + ir] || d.ctok[row + i] != d.ctok[row + ir]) { kind = JR_VERIFY_DIVERGED; id = x; break; }
+          if (x == 0 || nx < floor) break;
+          x = nx;
+        }
+      }
+    }
+    if (mine.x != VW_SKIP && (d.p2[i].w & 255u) == JR_ROLE_LEADER) {
+      const uint32_t term_lo = d.p0[i].x, term_hi = d.p0[i].y;
+      for (uint32_t k = 0; k < d.R; ++k) {
+        const size_t ik = (size_t)k * d.Gp + g;
+        if (vw[(size_t)k * n + j].x != VW_SKIP && (d.p2[ik].w & 255u) == JR_ROLE_LEADER && d.p0[ik].x == term_lo &&
+            d.p0[ik].y == term_hi)
+          lc |= 1u << k;
+      }
+      if (__popc(lc) < 2 || (lc & ((1u << r) - 1u))) lc = 0;   // reported once, by the lowest leader of the term
+    }
+    vf[t] = make_uint2(kind | (ref << 8) | (lc << 16), id);
+    cnt[0] = mine.x != VW_SKIP;
+    cnt[1] = mine.x == VW_SKIP;
+#pragma unroll
+    for (int c = 2; c < 6; ++c) cnt[c] = kind == (uint32_t)(c - 1);   // (static indices: the counts stay in registers)
+    cnt[6] = lc != 0;
+  }
+#ifdef JR_EMU
+  (void)s;
+  for (int c = 0; c < VERIFY_COUNTS; ++c)
+    if (cnt[c]) atomicAdd(rep + c, (unsigned long long)cnt[c]);
+#else
+#pragma unroll
+  for (int c = 0; c < VERIFY_COUNTS; ++c) {
+    uint64_t v = cnt[c];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) s[c][threadIdx.x >> 5] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < VERIFY_COUNTS) {
+    unsigned long long v = 0;
+    for (uint32_t w = 0; w < (blockDim.x + 31) / 32; ++w) v += s[threadIdx.x][w];
+    if (v) atomicAdd(rep + threadIdx.x, v);
+  }
+#endif
+}
+
+__device__ __forceinline__ uint32_t verify_findings_of(const Dev& d, const uint2* vf, uint32_t n, uint32_t j) {
+  uint32_t c = 0;
+  for (uint32_t k = 0; k < d.R; ++k) {
+    const uint32_t v = vf[(size_t)k * n + j].x;
+    c += ((v & 255u) != 0) + ((v >> 16) != 0);
+  }
+  return c;
+}
+
+// One thread per listed group: part[CTA] = the CTA's findings.
+__global__ void verify_count_kernel(const Dev d, uint32_t n, const uint2* vf, unsigned long long* part) {
+  __shared__ uint32_t s_warp[32];
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t c = j < n ? verify_findings_of(d, vf, n, j) : 0u;
+#ifdef JR_EMU
+  (void)s_warp;
+#else
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  c = 0;
+  for (uint32_t w = 0; w < (blockDim.x + 31) / 32; ++w) c += s_warp[w];
+#endif
+  part[blockIdx.x] = c;
+}
+
+// One thread: exclusive scan of the per-CTA counts (it only runs when some group has findings).
+__global__ void verify_scan_kernel(unsigned long long* part, uint32_t n_ctas) {
+  unsigned long long at = 0;
+  for (uint32_t k = 0; k < n_ctas; ++k) { const unsigned long long v = part[k]; part[k] = at; at += v; }
+}
+
+// One thread per listed group: its findings at part[CTA] + the CTA-local exclusive scan -- leader conflicts by their
+// lowest leader, then the replica findings by node.
+__global__ void verify_pack_kernel(const Dev d, const uint32_t* groups, uint32_t n, const uint2* vf,
+                                   const unsigned long long* part, jr_verify_finding* out) {
+  __shared__ uint32_t s_warp[32];
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t c = j < n ? verify_findings_of(d, vf, n, j) : 0u;
+  uint32_t pre = 0;
+#ifdef JR_EMU
+  (void)s_warp;
+#else
+  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+  uint32_t inc = c;
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= (uint32_t)o) inc += v;
+  }
+  if (lane == 31) s_warp[w] = inc;
+  __syncthreads();
+  uint32_t base = 0;
+  for (uint32_t k = 0; k < w; ++k) base += s_warp[k];
+  pre = base + inc - c;
+#endif
+  if (j >= n || c == 0) return;
+  const uint32_t g = verify_group(groups, j);
+  jr_verify_finding* o = out + part[blockIdx.x] + pre;
+  for (int pass = 0; pass < 2; ++pass)
+    for (uint32_t k = 0; k < d.R; ++k) {
+      const uint2 v = vf[(size_t)k * n + j];
+      const uint32_t kind = pass == 0 ? ((v.x >> 16) ? (uint32_t)JR_VERIFY_LEADER_CONFLICT : 0u) : (v.x & 255u);
+      if (!kind) continue;
+      const uint4 a = d.p0[(size_t)k * d.Gp + g];
+      jr_verify_finding f;
+      f.group = g;
+      f.kind = (uint8_t)kind;
+      f.node = pass == 0 ? 0 : (uint8_t)(k + 1);
+      f.ref_node = (uint8_t)((v.x >> 8) & 255u);
+      f.node_mask = (uint8_t)(pass == 0 ? (v.x >> 16) : (1u << k));
+      f.id = pass == 0 ? 0 : v.y;
+      f.term = (uint64_t)a.x | ((uint64_t)a.y << 32);
+      f.reserved = 0;
+      *o++ = f;
+    }
+}
+
 // ---- Instruction-stream drain -----------------------------------------------------------------
 // Records sit in per-replica FIFOs ([2*rec + half][replica][group]).  The drain packs them into one dense
 // array in thread order i = replica * Gp + group -- sorted by (node, group), FIFO per replica -- with an exclusive
@@ -1090,6 +1279,9 @@ struct jr_engine {
   // scratch of the *_many introspection calls (device, grows)
   void* many_buf = nullptr;
   size_t many_cap = 0;
+  // scratch of jr_verify_groups (device, grows; not part of a checkpoint): report, CTA offsets, group list, verdicts
+  void* verify_buf = nullptr;
+  size_t verify_cap = 0;
   // Instruction-stream drain (JR_F_CAPTURE_FSM): scan -> pack into stage[b] on the engine stream, then
   // fsm_copy_kernel moves stage[b] into the pinned host buffer host[b] on the d2h stream.
   unsigned long long* fsm_part = nullptr;                     // device, 3 x (CTAs of the count/pack kernels): per-CTA sums -> offsets
@@ -1545,6 +1737,7 @@ void jr_engine_destroy(jr_engine* e) {
   if (e->inj_msgs) cudaFree(e->inj_msgs);
   if (e->inj_targets) cudaFree(e->inj_targets);
   if (e->many_buf) cudaFree(e->many_buf);
+  if (e->verify_buf) cudaFree(e->verify_buf);
   if (e->h2d) { cudaStreamSynchronize(e->h2d); cudaStreamDestroy(e->h2d); }
   if (e->d2h) { cudaStreamSynchronize(e->d2h); cudaStreamDestroy(e->d2h); }
   for (int i = 0; i < jr_engine::NBUF; ++i) {
@@ -2419,16 +2612,19 @@ jr_status jr_fsm_expand(const jr_fsm_record* recs, size_t n_records, uint32_t G,
 
 // ---- introspection ----------------------------------------------------------------------------
 
-static jr_status many_reserve(jr_engine* e, size_t bytes) {
-  if (bytes <= e->many_cap) return JR_OK;
-  if (e->many_buf) cudaFree(e->many_buf);
-  e->many_buf = nullptr;
-  e->many_cap = 0;
+// Device scratch that grows on demand (contents are not kept).
+static jr_status scratch_reserve(void** buf, size_t* cap, size_t bytes) {
+  if (bytes <= *cap) return JR_OK;
+  if (*buf) cudaFree(*buf);
+  *buf = nullptr;
+  *cap = 0;
   const size_t want = std::max<size_t>(bytes * 2, 4096);
-  CK(cudaMalloc(&e->many_buf, want));
-  e->many_cap = want;
+  CK(cudaMalloc(buf, want));
+  *cap = want;
   return JR_OK;
 }
+
+static jr_status many_reserve(jr_engine* e, size_t bytes) { return scratch_reserve(&e->many_buf, &e->many_cap, bytes); }
 
 jr_status jr_query_many(jr_engine* e, const uint32_t* groups, const uint32_t* nodes, size_t n, jr_replica_state* out) {
   if (!e || !out || !groups || !nodes) return JR_E_INVAL;
@@ -2724,6 +2920,81 @@ jr_status jr_node_restart(jr_engine* e, uint32_t group, uint32_t node, uint64_t 
   c.n_blocks = (uint32_t)m;
   c.commit_key = commit_key ? 1u : 0u;
   return jr_node_restart_many(e, now_ms, &c, 1, v.data(), m);
+}
+
+jr_status jr_verify_groups(jr_engine* e, const uint32_t* groups, size_t n_groups, jr_verify_report* report,
+                           jr_verify_finding* findings, size_t cap, size_t* n_findings) {
+  if (!e || !report || !n_findings || (n_groups && !groups)) return JR_E_INVAL;
+  const Dev& d = e->d;
+  const size_t n = groups ? n_groups : d.G;
+  std::vector<uint32_t> list;
+  if (groups) {   // checked before the first device call: on JR_E_INVAL the engine is untouched
+    std::vector<uint8_t> seen(d.G, 0);
+    for (size_t k = 0; k < n; ++k) {
+      if (groups[k] >= d.G || seen[groups[k]]) {
+        set_err("groups[%zu]: out of range or named twice", k);
+        return JR_E_INVAL;
+      }
+      seen[groups[k]] = 1;
+    }
+    list.assign(groups, groups + n);
+    std::sort(list.begin(), list.end());   // findings come out in list order
+  }
+  memset(report, 0, sizeof *report);
+  report->groups_checked = n;
+  *n_findings = 0;
+  if (n == 0) return JR_OK;
+  CK(cudaSetDevice(e->cfg.device));
+#ifdef JR_EMU
+  const uint32_t T = 1;   // the CTA-wide scans of count and pack
+#else
+  const uint32_t T = 256;
+#endif
+  const size_t reps = (size_t)d.R * n;
+  const uint32_t n_ctas = (uint32_t)((n + T - 1) / T);
+  const size_t o_part = 16 * sizeof(unsigned long long), o_list = o_part + ((size_t)n_ctas * 8 + 15) / 16 * 16;
+  const size_t o_vw = o_list + (n * 4 + 15) / 16 * 16, o_vf = o_vw + reps * sizeof(uint2);
+  jr_status st = scratch_reserve(&e->verify_buf, &e->verify_cap, o_vf + reps * sizeof(uint2));
+  if (st != JR_OK) return st;
+  char* base = (char*)e->verify_buf;
+  unsigned long long* rep = (unsigned long long*)base;
+  unsigned long long* part = (unsigned long long*)(base + o_part);
+  const uint32_t* dlist = groups ? (const uint32_t*)(base + o_list) : nullptr;   // null: group = list index
+  uint2* vw = (uint2*)(base + o_vw);
+  uint2* vf = (uint2*)(base + o_vf);
+  CK(cudaMemsetAsync(rep, 0, VERIFY_COUNTS * sizeof(unsigned long long), e->stream));
+  if (groups) CK(cudaMemcpyAsync(base + o_list, list.data(), n * 4, cudaMemcpyHostToDevice, e->stream));
+  const unsigned grid = (unsigned)((reps + 255) / 256);
+  JR_LAUNCH(verify_walk_kernel, grid, 256, e->stream, d, dlist, (uint32_t)n, vw);
+  CK(cudaGetLastError());
+  JR_LAUNCH(verify_judge_kernel, grid, 256, e->stream, d, dlist, (uint32_t)n, (const uint2*)vw, vf, rep);
+  CK(cudaGetLastError());
+  unsigned long long cnt[VERIFY_COUNTS];
+  CK(cudaMemcpyAsync(cnt, rep, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));   // (also covers `list`)
+  report->replicas_checked = cnt[0];
+  report->replicas_skipped = cnt[1];
+  report->below_floor = cnt[2];
+  report->commit_absent = cnt[3];
+  report->chain_broken = cnt[4];
+  report->diverged = cnt[5];
+  report->leader_conflicts = cnt[6];
+  const size_t total = (size_t)(cnt[2] + cnt[3] + cnt[4] + cnt[5] + cnt[6]);
+  *n_findings = total;
+  if (total == 0) return JR_OK;
+  if (!findings || cap < total) return JR_E_CAPACITY;
+  // something to report: count, scan and pack the findings in (group, node) order on the device, then one copy
+  if ((st = many_reserve(e, total * sizeof(jr_verify_finding))) != JR_OK) return st;
+  jr_verify_finding* out = (jr_verify_finding*)e->many_buf;
+  JR_LAUNCH(verify_count_kernel, n_ctas, T, e->stream, d, (uint32_t)n, (const uint2*)vf, part);
+  CK(cudaGetLastError());
+  JR_LAUNCH(verify_scan_kernel, 1, 1, e->stream, part, n_ctas);
+  CK(cudaGetLastError());
+  JR_LAUNCH(verify_pack_kernel, n_ctas, T, e->stream, d, dlist, (uint32_t)n, (const uint2*)vf, (const unsigned long long*)part, out);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(findings, out, total * sizeof(jr_verify_finding), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
 }
 
 // ---- checkpoint -----------------------------------------------------------------------------------

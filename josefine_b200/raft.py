@@ -478,6 +478,26 @@ class RaftApi:
         self._check(self._fn("node_restart_many")(self._h, C.c_uint64(now_ms), desc, C.c_size_t(n), arr,
                                                   C.c_size_t(len(flat))), "node_restart_many")
 
+    def verify_groups(self, groups: Optional[Sequence[int]] = None) -> Tuple[abi.VerifyReport, List[abi.VerifyFinding]]:
+        """jr_verify_groups: check that each group's replicas hold the same committed chain (None = every group).
+        Returns (report, findings), findings sorted by (group, node); an empty list means every checked replica agrees.
+        Without the batched call (the oracle): the same rules restated over query_many / chain_read_many (verify.py)."""
+        if not hasattr(self._lib, self._p + "verify_groups"):
+            from .verify import verify_groups
+            return verify_groups(self, groups)
+        n = 0 if groups is None else len(groups)
+        gs = None if groups is None else (C.c_uint32 * max(n, 1))(*groups)
+        rep, need = abi.VerifyReport(), C.c_size_t(0)
+        fn = self._fn("verify_groups")
+        st = fn(self._h, gs, C.c_size_t(n), C.byref(rep), None, C.c_size_t(0), C.byref(need))
+        if st == abi.OK:
+            return rep, []
+        if st != abi.E_CAPACITY:
+            self._check(st, "verify_groups")
+        buf = (abi.VerifyFinding * need.value)()
+        self._check(fn(self._h, gs, C.c_size_t(n), C.byref(rep), buf, need, C.byref(need)), "verify_groups")
+        return rep, [buf[i] for i in range(need.value)]
+
     def save(self) -> bytes:
         """jr_engine_save: checkpoint of everything the engine holds."""
         n = C.c_size_t(0)
@@ -569,6 +589,8 @@ def _bind(lib: C.CDLL, p: str):
         "chain_export_many": [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(abi.PersistedChain),
                               C.POINTER(abi.Block), C.c_size_t, C.POINTER(C.c_size_t)],
         "node_restart_many": [vp, C.c_uint64, C.POINTER(abi.PersistedChain), C.c_size_t, C.POINTER(abi.Block), C.c_size_t],
+        "verify_groups": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(abi.VerifyReport), C.POINTER(abi.VerifyFinding),
+                          C.c_size_t, C.POINTER(C.c_size_t)],
         "engine_save_size": [vp, C.POINTER(C.c_size_t)],
         "engine_save": [vp, C.c_void_p, C.c_size_t],
         "engine_restore": [vp, C.c_void_p, C.c_size_t],

@@ -89,3 +89,13 @@ for fl in (0, abi.F_NO_SYMMETRIC_FOLD):
     e.drain_fsm()
     print("client responses", fl, answered, e.fsm_responses()[1].n_instructions)
 print("client-response sanitize workload done")
+
+# replica verification: every group, then a subset, with findings to pack (one follower restarted from a doctored export)
+e = RaftEngine.create(64, 5, seed=9, chain_capacity=64)
+e.step(0, flags=0, inject=bootstrap(64, 5))
+e.run(100, 100, 20, 1)
+c, ck, bl = e.chain_export_many([(5, 2)])[0]
+e.node_restart_many(2100, [(5, 2, [(i, n, t + (i == c - 1)) for i, n, t in bl], c, ck)])
+rep, findings = e.verify_groups()
+print("verify", rep.as_tuple(), [f.as_tuple() for f in findings], len(e.verify_groups([9, 5, 0])[1]))
+print("verify sanitize workload done")
