@@ -1284,19 +1284,23 @@ struct jr_engine {
   size_t verify_cap = 0;
   // Instruction-stream drain (JR_F_CAPTURE_FSM): scan -> pack into stage[b] on the engine stream, then
   // fsm_copy_kernel moves stage[b] into the pinned host buffer host[b] on the d2h stream.
+  // One slot more than batches may be outstanding, used round robin: with NBUF batches outstanding at a
+  // jr_fsm_records_wait, the next enqueue goes to the spare slot, so the batch just returned is reused no earlier
+  // than the second enqueue after the wait (the lifetime the ABI header promises), and never while its take runs.
+  static constexpr int NSLOT = NBUF + 1;
   unsigned long long* fsm_part = nullptr;                     // device, 3 x (CTAs of the count/pack kernels): per-CTA sums -> offsets
   uint32_t fsm_cap = 0;                                       // records per batch
-  uint4* fsm_stage[NBUF] = {nullptr, nullptr};                // device, 2 * fsm_cap uint4 each
-  FsmHeader* fsm_stage_hdr[NBUF] = {nullptr, nullptr};        // device
-  uint4* fsm_host[NBUF] = {nullptr, nullptr};                 // pinned + mapped host
-  FsmHeader* fsm_host_hdr[NBUF] = {nullptr, nullptr};         // pinned + mapped host
-  cudaEvent_t fsm_packed[NBUF] = {nullptr, nullptr};          // pack into stage[b] finished (engine stream)
-  cudaEvent_t fsm_landed[NBUF] = {nullptr, nullptr};          // copy into host[b] finished (d2h stream)
-  size_t fsm_copied[NBUF] = {0, 0};                           // records of stage[b] the enqueued copy covers
+  uint4* fsm_stage[NSLOT] = {};                               // device, 2 * fsm_cap uint4 each
+  FsmHeader* fsm_stage_hdr[NSLOT] = {};                       // device
+  uint4* fsm_host[NSLOT] = {};                                // pinned + mapped host
+  FsmHeader* fsm_host_hdr[NSLOT] = {};                        // pinned + mapped host
+  cudaEvent_t fsm_packed[NSLOT] = {};                         // pack into stage[b] finished (engine stream)
+  cudaEvent_t fsm_landed[NSLOT] = {};                         // copy into host[b] finished (d2h stream)
+  size_t fsm_copied[NSLOT] = {};                              // records of stage[b] the enqueued copy covers
   size_t fsm_last_records = 0;                                // size of the last batch taken (the next copy's guess)
   int fsm_copy_by_sm = 0;                                     // JR_FSM_COPY=sm (A/B): fsm_copy_kernel instead of the copy engine
-  bool fsm_used[NBUF] = {false, false};
-  int fsm_i = 0, fsm_pending[NBUF] = {0, 0}, fsm_npending = 0;
+  bool fsm_used[NSLOT] = {};
+  int fsm_i = 0, fsm_pending[NBUF] = {0, 0}, fsm_npending = 0;   // at most NBUF batches outstanding
   std::mutex qmu;   // the two FIFOs of outstanding copy-outs (fsm_pending, tab_pending) and fsm_last_records: a second host thread may
                     // sit in jr_fsm_records_wait / jr_leader_table_wait while the first one keeps submitting
   uint32_t fsm_epoch = 0;
@@ -1304,7 +1308,7 @@ struct jr_engine {
   // record fsm_cap on) with their header at fsm_stage_hdr[b][1] / fsm_host_hdr[b][1]
   RespPlanes rp = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   uint32_t resp_cap = 0;
-  size_t resp_copied[NBUF] = {0, 0};
+  size_t resp_copied[NSLOT] = {};
   size_t resp_last = 0;                                       // size of the last response batch taken (the next copy's guess)
   int resp_b = -1;                                            // buffer of the batch most recently taken (-1: none yet)
   // symmetric-group fold
@@ -1604,7 +1608,7 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
     }
     const size_t n_hdr = e->resp_cap ? 2 : 1;
     A(e->fsm_part, 3 * plane);   // (sized for one-thread CTAs, which is what the CPU emulation launches)
-    for (int i = 0; i < jr_engine::NBUF; ++i) {
+    for (int i = 0; i < jr_engine::NSLOT; ++i) {
       A(e->fsm_stage[i], 2 * ((size_t)e->fsm_cap + e->resp_cap));
       A(e->fsm_stage_hdr[i], n_hdr);
     }
@@ -1634,10 +1638,11 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
            cudaEventCreateWithFlags(&e->tab_ready[i], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&e->tab_free[i], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&e->batch_ready[i], cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&e->batch_free[i], cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&e->fsm_packed[i], cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&e->batch_free[i], cudaEventDisableTiming) == cudaSuccess;
+    for (int i = 0; ok && i < jr_engine::NSLOT; ++i)
+      ok = cudaEventCreateWithFlags(&e->fsm_packed[i], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&e->fsm_landed[i], cudaEventDisableTiming) == cudaSuccess;
-    for (int i = 0; ok && e->fsm_cap && i < jr_engine::NBUF; ++i)   // the drain's landing buffers: pinned, device-visible
+    for (int i = 0; ok && e->fsm_cap && i < jr_engine::NSLOT; ++i)   // the drain's landing buffers: pinned, device-visible
       ok = cudaHostAlloc((void**)&e->fsm_host[i], ((size_t)e->fsm_cap + e->resp_cap) * sizeof(jr_fsm_record), cudaHostAllocMapped) == cudaSuccess &&
            cudaHostAlloc((void**)&e->fsm_host_hdr[i], (e->resp_cap ? 2 : 1) * sizeof(FsmHeader), cudaHostAllocMapped) == cudaSuccess;
     if (!ok) {
@@ -1747,12 +1752,14 @@ void jr_engine_destroy(jr_engine* e) {
     if (e->tab_free[i]) cudaEventDestroy(e->tab_free[i]);
     if (e->batch_ready[i]) cudaEventDestroy(e->batch_ready[i]);
     if (e->batch_free[i]) cudaEventDestroy(e->batch_free[i]);
+    if (e->batch[i]) cudaFree(e->batch[i]);
+    if (e->tokbuf[i]) cudaFree(e->tokbuf[i]);
+  }
+  for (int i = 0; i < jr_engine::NSLOT; ++i) {
     if (e->fsm_packed[i]) cudaEventDestroy(e->fsm_packed[i]);
     if (e->fsm_landed[i]) cudaEventDestroy(e->fsm_landed[i]);
     if (e->fsm_host[i]) cudaFreeHost(e->fsm_host[i]);
     if (e->fsm_host_hdr[i]) cudaFreeHost(e->fsm_host_hdr[i]);
-    if (e->batch[i]) cudaFree(e->batch[i]);
-    if (e->tokbuf[i]) cudaFree(e->tokbuf[i]);
   }
   if (e->h_scatter) cudaFreeHost((void*)e->h_scatter);
   if (e->h_unfolded) cudaFreeHost((void*)e->h_unfolded);
@@ -1860,7 +1867,7 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
     last_resp = e->resp_last;
   }
   const int b = e->fsm_i;
-  e->fsm_i = (b + 1) % jr_engine::NBUF;
+  e->fsm_i = (b + 1) % jr_engine::NSLOT;
   const size_t plane = (size_t)d.R * d.Gp;
   if (e->fsm_used[b]) CK(cudaStreamWaitEvent(e->stream, e->fsm_landed[b], 0));  // stage[b] has left the device
   const uint32_t epoch = ++e->fsm_epoch;
@@ -3156,6 +3163,7 @@ jr_status jr_leader_table(jr_engine* e, jr_leader_entry* host_out) {
   jr_status st = jr_leader_table_async(e, host_out);
   if (st != JR_OK) return st;
   CK(cudaStreamSynchronize(e->d2h));
+  std::lock_guard<std::mutex> l(e->qmu);   // a consumer thread may sit in jr_leader_table_wait
   e->tab_npending = 0;
   return JR_OK;
 }
