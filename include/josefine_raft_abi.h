@@ -52,7 +52,11 @@
  *   D3  panics / Err returns of the reference become a sticky per-replica
  *       fault code (JR_FAULT_*); a faulted replica stops like a dead process.
  *   D4  node ids are 1..65534 (reference: any non-zero u32, config.rs:64);
- *       block ids must be < chain_capacity (reference: any u64).
+ *       block ids lie in [floor, floor + chain_capacity) (D7; floor 0 without
+ *       truncation) and below 2^31 = JR_BLOCK_ID_LIMIT (reference: any u64).  An
+ *       append or extend that would store an id outside that range faults the
+ *       replica with JR_FAULT_ENGINE_CHAIN_CAPACITY; with truncation the ids keep
+ *       growing, so a group reaches 2^31 after 2^31 appends.
  *   D5  Block.data (Vec<u8>) is represented on the device by a 64-bit token the
  *       host maps to the payload bytes; ClientRequest.id (Uuid) likewise.
  *   D6  the sled "commit" key shares the block keyspace in the reference
@@ -88,6 +92,7 @@ extern "C" {
 #define JR_STAGING_DEPTH 3u       /* steps a host may keep in flight on the async paths */
 #define JR_MAX_AE_BLOCKS 5u       /* MAX_INFLIGHT, src/raft/progress.rs:117          */
 #define JR_MAX_NODE_ID 65534u     /* deviation D4                                    */
+#define JR_BLOCK_ID_LIMIT 0x80000000u  /* block ids are below 2^31 (deviation D4)    */
 #define JR_CLIENT_QUEUE_CAP 4u    /* queued_reqs bound per replica (reference: Vec)  */
 #define JR_NOTIFY_RUNS 8u         /* pending-notification runs per replica with JR_F_CLIENT_RESPONSES
                                    * (reference: the Driver's unbounded HashMap, fsm.rs:36,78-81) */
@@ -138,7 +143,7 @@ enum {
   JR_FAULT_CANDIDATE_TICK_ELECTED = 7,/* panic!("this should never happen"), candidate.rs:63 */
   JR_FAULT_RANGE_COMMIT_KEY = 8,      /* bincode panic on the "commit" key, chain.rs:222-226 (D6) */
   /* 64..: engine limits, not reference behaviour */
-  JR_FAULT_ENGINE_CHAIN_CAPACITY = 64,   /* block id outside [floor, floor + chain_capacity) (D4, D7) */
+  JR_FAULT_ENGINE_CHAIN_CAPACITY = 64,   /* block id outside [floor, floor + chain_capacity) or >= 2^31 (D4, D7) */
   JR_FAULT_ENGINE_MAILBOX_OVERFLOW = 65, /* a replica emitted more than mailbox_units units  */
   JR_FAULT_ENGINE_FSM_OVERFLOW = 66,     /* retired in ABI 2: a full Instruction FIFO drops records and the drain
                                           * returns JR_E_CAPACITY; observing a node never changes consensus     */
@@ -499,7 +504,8 @@ jr_status jr_fsm_fold_mt(const jr_fsm_record* records, size_t n_records, uint32_
 
 /* ---- introspection --------------------------------------------------------- */
 jr_status jr_query(jr_engine* e, uint32_t group, uint32_t node, jr_replica_state* out);
-/* blocks with first_id <= id < first_id+n of one replica; present[i]=0 if absent. */
+/* blocks with first_id <= id < first_id+n of one replica; present[i]=0 if absent.  JR_E_INVAL unless
+ * first_id + n <= 2^32-1 (in exact arithmetic: a first_id near 2^64 is refused, not wrapped). */
 jr_status jr_chain_read(jr_engine* e, uint32_t group, uint32_t node, uint64_t first_id,
                         uint32_t n, jr_block* out, uint8_t* present);
 /* The same for n replicas in ONE kernel + ONE copy: replica i is (groups[i], nodes[i]). */
@@ -534,7 +540,8 @@ jr_status jr_set_auto_truncate(jr_engine* e, int enabled, uint32_t margin);
  * Node restart: replica (group, node) becomes what RaftHandle::new builds over an existing data directory
  * (mod.rs:428-435 -> follower.rs:68-95 -> Chain::new, chain.rs:117-137): a Follower with State::default
  * (term 0, voted_for None -- the reference does not persist them), election timer started at now_ms,
- * the block table = `blocks`, commit = head = id_gen = `commit` (so the first append of a restarted
+ * the block table = `blocks` (ids, their `next` and `commit` below 2^31, D4), commit = head = id_gen = `commit`
+ * (so the first append of a restarted
  * leader-to-be asserts id > head and faults, SURVEY note N2).  commit == 0 runs Chain::init (genesis
  * block 0 -> 0 is (re)written, id_gen = 1).  `commit_key` = the sled "commit" key exists (D6).
  * The replica's mailbox and client queue are emptied; it is alive and unfaulted afterwards.
@@ -569,8 +576,10 @@ jr_status jr_chain_export_many(jr_engine* e, const uint32_t* groups, const uint3
  * every block and commit through to sled) -- the same as exporting it and restarting from the export; first_block,
  * commit and commit_key are then ignored.  All or nothing: JR_E_INVAL, engine untouched, unless every group / node
  * is in range, no (group, node) appears twice, every slice lies inside `blocks` and holds at most chain_capacity
- * blocks with strictly ascending ids inside [floor, floor + chain_capacity) and next < 2^32-1, and every
- * commit < 2^32-1.  Synchronous.
+ * blocks with strictly ascending ids inside [floor, floor + chain_capacity), and every block id, every next and
+ * every commit is below 2^31 (D4: a `next` names a parent block, so it obeys the same limit; no engine can have
+ * written one at or above it).  Once a group's floor is within chain_capacity of 2^31 its window straddles the
+ * limit, and the ids at or above 2^31 in it are refused.  Synchronous.
  */
 jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted_chain* chains, size_t n,
                                const jr_block* blocks, size_t n_blocks);

@@ -2668,7 +2668,7 @@ jr_status jr_chain_read_many(jr_engine* e, const uint32_t* groups, const uint32_
   size_t total = 0;
   for (size_t i = 0; i < n; ++i) {
     if (groups[i] >= e->d.G || nodes[i] < 1 || nodes[i] > e->d.R) return JR_E_INVAL;
-    if (first_id[i] + count[i] > 0xffffffffull) return JR_E_INVAL;
+    if (first_id[i] > 0xffffffffull - count[i]) return JR_E_INVAL;   // ids past 2^32-2 (no wrap: count < 2^32)
     reqs[i] = make_uint4(groups[i], nodes[i] - 1, (uint32_t)first_id[i], (uint32_t)total);
     total += count[i];
     if (total > 0xffffffffull) return JR_E_INVAL;
@@ -2871,8 +2871,8 @@ jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted
     }
     s = 1;
     if (c.n_blocks == JR_RESTART_IN_PLACE) continue;
-    if (c.n_blocks > d.cap || c.first_block > n_blocks || n_blocks - c.first_block < c.n_blocks || c.commit >= 0xffffffffull) {
-      set_err("chains[%zu]: slice outside blocks[0, %zu), more than chain_capacity blocks, or commit >= 2^32-1", k, n_blocks);
+    if (c.n_blocks > d.cap || c.first_block > n_blocks || n_blocks - c.first_block < c.n_blocks || c.commit >= JR_BLOCK_ID_LIMIT) {
+      set_err("chains[%zu]: slice outside blocks[0, %zu), more than chain_capacity blocks, or commit >= 2^31 (D4)", k, n_blocks);
       return JR_E_INVAL;
     }
     host_blocks |= c.n_blocks > 0;
@@ -2888,8 +2888,9 @@ jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted
       const uint64_t lo = floor[c.group - g_lo];
       for (uint32_t j = 0; j < c.n_blocks; ++j) {
         const jr_block& b = blocks[c.first_block + j];
-        if (b.id < lo || b.id - lo >= d.cap || b.next >= 0xffffffffull || (j && b.id <= blocks[c.first_block + j - 1].id)) {
-          set_err("chains[%zu] block %u: id not ascending or outside [floor, floor + chain_capacity), or next >= 2^32-1 (D4, D7)", k, j);
+        if (b.id < lo || b.id - lo >= d.cap || b.id >= JR_BLOCK_ID_LIMIT || b.next >= JR_BLOCK_ID_LIMIT ||
+            (j && b.id <= blocks[c.first_block + j - 1].id)) {
+          set_err("chains[%zu] block %u: id not ascending, outside [floor, floor + chain_capacity) or >= 2^31, or next >= 2^31 (D4, D7)", k, j);
           return JR_E_INVAL;
         }
       }
@@ -2913,7 +2914,7 @@ jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted
 jr_status jr_node_restart(jr_engine* e, uint32_t group, uint32_t node, uint64_t now_ms, const jr_block* blocks,
                           size_t n_blocks, uint64_t commit, int commit_key) {
   if (!e || group >= e->d.G || node < 1 || node > e->d.R || (n_blocks && !blocks)) return JR_E_INVAL;
-  if (n_blocks > e->d.cap || commit >= 0xffffffffull) return JR_E_INVAL;
+  if (n_blocks > e->d.cap || commit >= JR_BLOCK_ID_LIMIT) return JR_E_INVAL;
   std::vector<jr_block> v(blocks, blocks + n_blocks);
   std::stable_sort(v.begin(), v.end(), [](const jr_block& a, const jr_block& b) { return a.id < b.id; });
   size_t m = 0;

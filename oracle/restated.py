@@ -37,6 +37,7 @@ def load() -> C.CDLL:
         lib.jro_create.restype = C.c_int
         lib.jro_destroy.argtypes = [C.c_void_p]
         lib.jro_destroy.restype = None
+        lib.jro_shift_ids.argtypes, lib.jro_shift_ids.restype = [C.c_void_p, C.c_uint64], C.c_int
         # direct Chain access for the ported chain.rs tests
         vp, u64 = C.c_void_p, C.c_uint64
         lib.jro_chain_new.argtypes, lib.jro_chain_new.restype = [u64, C.c_int], vp
@@ -71,6 +72,10 @@ class RestatedCluster(RaftApi):
     @classmethod
     def create(cls, n_groups: int, n_replicas: int, n_threads: int = 1, **kw) -> "RestatedCluster":
         return cls(abi.default_config(n_groups, n_replicas, **kw), n_threads)
+
+    def shift_ids(self, k: int):
+        """jro_shift_ids (test-only): every group's ids at or above its floor move up by k; needs a quiet cluster."""
+        self._check(self._lib.jro_shift_ids(self._h, C.c_uint64(k)), "shift_ids")
 
 
 class RestatedChain:

@@ -641,9 +641,11 @@ jr_status jro_node_restart(jro_cluster* c, uint32_t group, uint32_t node, uint64
   if (!c || group >= c->cfg.n_groups || node < 1 || node > c->cfg.n_replicas || (n_blocks && !blocks)) return JR_E_INVAL;
   Replica& rep = c->at(group, node);
   const uint64_t floor = rep.node->chain.floor();
+  if (commit >= JR_BLOCK_ID_LIMIT) return JR_E_INVAL;  // D4
   std::vector<Block> persisted;
   for (size_t k = 0; k < n_blocks; ++k) {
     if (blocks[k].id < floor || blocks[k].id - floor >= c->cfg.chain_capacity) return JR_E_INVAL;
+    if (blocks[k].id >= JR_BLOCK_ID_LIMIT || blocks[k].next >= JR_BLOCK_ID_LIMIT) return JR_E_INVAL;  // D4
     persisted.push_back(Block{blocks[k].id, blocks[k].next, blocks[k].data});
   }
   NodeConfig nc = rep.node->config();
@@ -652,6 +654,43 @@ jr_status jro_node_restart(jro_cluster* c, uint32_t group, uint32_t node, uint64
   rep.node = std::make_unique<Node>(nc, Chain(c->cfg.chain_capacity, strict, persisted, commit, commit_key != 0, floor), now_ms);
   rep.node->fsm = std::move(undrained);
   rep.prev_out.clear();
+  return JR_OK;
+}
+
+// Test-only: moves every group's block ids up by k with f(v) = v + k for v >= F, v for v < F, F = the group's floor.
+// f keeps every order, equality and the literal 0 (F > 0), and commutes with what Raft does with ids, so the shifted
+// cluster's future is the old one's future shifted by f -- until an id reaches 2^31 (D4).  Only between steps with no
+// mail and no undrained Instruction (they carry ids too), every floor above 0 and every shifted id below 2^31;
+// JR_E_INVAL otherwise, with nothing changed.
+jr_status jro_shift_ids(jro_cluster* c, uint64_t k) {
+  if (!c) return JR_E_INVAL;
+  const uint32_t R = c->cfg.n_replicas;
+  for (uint32_t g = 0; g < c->cfg.n_groups; ++g) {
+    const uint64_t floor = c->at(g, 1).node->chain.floor();
+    if (floor == 0 || k >= JR_BLOCK_ID_LIMIT) return JR_E_INVAL;
+    auto bad = [&](uint64_t v) { return v >= floor && v + k >= JR_BLOCK_ID_LIMIT; };
+    for (uint32_t r = 1; r <= R; ++r) {
+      const Replica& rep = c->at(g, r);
+      const Node& n = *rep.node;
+      const Chain& ch = n.chain;
+      if (!rep.prev_out.empty() || !n.rpc.empty() || !n.fsm.empty() || ch.floor() != floor) return JR_E_INVAL;
+      if (bad(floor) || bad(ch.get_head()) || bad(ch.get_commit()) || bad(ch.id_gen())) return JR_E_INVAL;
+      for (auto& kv : ch.blocks())
+        if (bad(kv.first) || bad(kv.second.next)) return JR_E_INVAL;
+      if (n.progress)
+        for (auto& kv : n.progress->all())
+          if (bad(kv.second.head)) return JR_E_INVAL;
+    }
+  }
+  for (uint32_t g = 0; g < c->cfg.n_groups; ++g)
+    for (uint32_t r = 1; r <= R; ++r) {
+      Node& n = *c->at(g, r).node;
+      const uint64_t floor = n.chain.floor();
+      n.chain.shift_ids(k);
+      if (n.progress)
+        for (auto& kv : n.progress->all_mut())
+          if (kv.second.head >= floor) kv.second.head += k;
+    }
   return JR_OK;
 }
 

@@ -46,7 +46,18 @@ Chain::Chain(uint64_t capacity, bool strict, const std::vector<Block>& persisted
 }
 
 void Chain::check_capacity(BlockId id) const {
-  if (id < floor_ || id - floor_ >= capacity_) throw Fault{JR_FAULT_ENGINE_CHAIN_CAPACITY};  // D4, D7
+  if (id < floor_ || id - floor_ >= capacity_ || id >= JR_BLOCK_ID_LIMIT) throw Fault{JR_FAULT_ENGINE_CHAIN_CAPACITY};  // D4, D7
+}
+
+void Chain::shift_ids(uint64_t k) {  // test-only: f(v) = v + k for v >= floor, v below it unchanged
+  auto f = [&](BlockId v) { return v >= floor_ ? v + k : v; };
+  std::map<BlockId, Block> db;
+  for (auto& kv : db_) db[f(kv.first)] = Block{f(kv.second.id), f(kv.second.next), kv.second.data};
+  db_.swap(db);
+  id_gen_ = f(id_gen_);
+  commit_ = f(commit_);
+  head_ = f(head_);
+  floor_ += k;
 }
 
 void Chain::truncate(BlockId floor) {  // D7

@@ -94,6 +94,7 @@ class Chain {
   Chain(uint64_t capacity, bool strict_commit_key, const std::vector<Block>& persisted, uint64_t commit, bool commit_key,
         uint64_t floor);
   void truncate(BlockId floor);                              // deviation D7: keys below `floor` leave the tree
+  void shift_ids(uint64_t k);                                // test-only (jro_shift_ids): ids >= floor move up by k
   BlockId floor() const { return floor_; }
   bool has(BlockId id) const;                                // chain.rs:155-157
   BlockId append(uint64_t data);                             // chain.rs:160-175
@@ -151,6 +152,7 @@ class ReplicationProgress {
  public:
   explicit ReplicationProgress(const std::vector<NodeId>& nodes);  // progress.rs:15-23
   NodeProgress* get_mut(NodeId id);                                // progress.rs:29-31
+  std::map<NodeId, NodeProgress>& all_mut() { return progress_; }  // test-only (jro_shift_ids)
   void advance(NodeId id, BlockId block);                          // progress.rs:42-46
   BlockId committed_index() const;                                 // progress.rs:48-60
   const std::map<NodeId, NodeProgress>& all() const { return progress_; }

@@ -19,15 +19,16 @@ QUEUE_CAP = 4                                   # JR_CLIENT_QUEUE_CAP
 class Checkpoint:
     """Numpy views of the state planes inside a jr_engine_save blob (segment order of save_segments, engine.cu)."""
 
-    def __init__(self, blob):
+    def __init__(self, blob, G=G, R=R, cfg=CFG):
         self.buf = bytearray(blob)
+        self.G, self.R = G, R
         Gp = -(-G // 32) * 32
         self.Gp, plane = Gp, R * Gp
         rows = 1
-        while rows < CFG["chain_capacity"]:
+        while rows < cfg["chain_capacity"]:
             rows *= 2
         self.rows = rows
-        U, F = CFG["mailbox_units"], CFG["fsm_units"]
+        U, F = cfg["mailbox_units"], cfg["fsm_units"]
         segs = [("p0", plane * 4, np.uint32), ("p1", plane * 4, np.uint32), ("p2", plane * 4, np.uint32),
                 ("p3", plane * 4, np.uint32), ("pr", plane * ((R + 3) // 4) * 4, np.uint32), ("mk", plane, np.uint32),
                 ("qt", plane * QUEUE_CAP * 4, np.uint32), ("dg", plane * 4, np.uint32), ("cn", plane * 2, np.uint32),
@@ -35,6 +36,9 @@ class Checkpoint:
                 ("ob0", plane * U * 4, np.uint32), ("ob1", plane * U * 4, np.uint32),
                 ("oc0", plane, np.uint32), ("oc1", plane, np.uint32), ("fs", plane * 2 * F * 4, np.uint32),
                 ("fc", plane * 2, np.uint32), ("tb", Gp, np.uint32), ("route", G, np.uint32)]
+        if cfg.get("flags", 0) & abi.F_CLIENT_RESPONSES:            # the Driver maps: runs, run counts, restart marks
+            segs += [("pn", 2 * abi.NOTIFY_RUNS * plane * 4, np.uint32), ("pnc", -(-plane // 4) * 4, np.uint32),
+                     ("rm", plane * 4, np.uint32)]
         total = sum(n * np.dtype(t).itemsize for _, n, t in segs)
         at = len(self.buf) - total                # the header's size
         self.cur = int(np.frombuffer(self.buf, np.uint32, 1, at - 16)[0])
@@ -48,14 +52,14 @@ class Checkpoint:
 
     def unit(self, buf, k, r, g):                 # outbox unit k of replica r: a writable uint4 view
         ob = self.ob0 if buf == 0 else self.ob1
-        i = ((k * R + r) * self.Gp + g) * 4
+        i = ((k * self.R + r) * self.Gp + g) * 4
         return ob[i:i + 4]
 
     def count(self, buf, r, g):
         return int((self.oc0 if buf == 0 else self.oc1)[self.rg(r, g)])
 
     def row(self, r, bid, g):
-        return (bid & (self.rows - 1)) * R * self.Gp + self.rg(r, g)
+        return (bid & (self.rows - 1)) * self.R * self.Gp + self.rg(r, g)
 
 
 def _quad(a, r, g, ck):
