@@ -1619,6 +1619,9 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
 #ifdef JR_PROFILE
   A(d.prof, 3 * 16 * 2);
 #endif
+#ifdef JR_SYM_ABORT_LOG
+  A(d.sab, 2 * (size_t)d.Gp);
+#endif
   for (int i = 0; i < jr_engine::NBUF; ++i) { A(e->prop[i], d.G); A(e->leaders[i], d.G); }
   A(e->route, d.G);
 #undef A
@@ -1702,6 +1705,21 @@ jr_status jr_profile_read(jr_engine* e, unsigned long long* out96) {
 }
 #endif
 
+#ifdef JR_SYM_ABORT_LOG
+// Abort-log builds only (tests/emu; not part of the ABI): read and clear the fold's abort records, out[lane * G + g] =
+// the first abort site | tick << 8 of group g's lane since the last read, 0 = none (sym_fold.cuh, SA_*).
+jr_status jr_sym_abort_read(jr_engine* e, uint32_t* out, size_t n) {
+  if (!e || !out || n < 2 * (size_t)e->d.G) return JR_E_INVAL;
+  CK(cudaStreamSynchronize(e->stream));
+  for (int lane = 0; lane < 2; ++lane)
+    CK(cudaMemcpyAsync(out + (size_t)lane * e->d.G, e->d.sab + (size_t)lane * e->d.Gp, e->d.G * sizeof(uint32_t),
+                       cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemsetAsync(e->d.sab, 0, 2 * (size_t)e->d.Gp * sizeof(uint32_t), e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
+}
+#endif
+
 jr_status jr_engine_reset(jr_engine* e) {
   if (!e) return JR_E_INVAL;
   CK(cudaSetDevice(e->cfg.device));
@@ -1726,6 +1744,9 @@ jr_status jr_engine_reset(jr_engine* e) {
   // (h_scatter keeps its last value: advisory only, and a reset is usually followed by the same workload)
 #ifdef JR_PROFILE
   CK(cudaMemsetAsync(e->d.prof, 0, 96 * sizeof(unsigned long long), e->stream));
+#endif
+#ifdef JR_SYM_ABORT_LOG
+  CK(cudaMemsetAsync(e->d.sab, 0, 2 * (size_t)d.Gp * sizeof(uint32_t), e->stream));
 #endif
   return JR_OK;
 }

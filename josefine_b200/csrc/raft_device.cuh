@@ -66,6 +66,9 @@ struct Dev {
                                    // [1] task ticket counter of the running step launch (both zeroed per launch)
   uint32_t* done;                  // [CTA-sized group block]: epoch + parts finished (split launches, see step_kernel)
   unsigned long long* prof;        // JR_PROFILE builds: cycle counters [role 3][slot 16] x {cycles, count}
+#ifdef JR_SYM_ABORT_LOG
+  uint32_t* sab;                   // [lane 2][group]: the fold's first abort site | tick << 8 (sym_fold.cuh, SA_*)
+#endif
   uint64_t seed, goff;
 };
 

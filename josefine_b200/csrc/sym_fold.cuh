@@ -30,6 +30,8 @@
 //     created with that flag, or with JR_F_SLED_COMMIT_KEY_STRICT / JR_F_NO_SYMMETRIC_FOLD, never take it.
 //     tests/test_sym_fold.py compares folded runs with step_kernel runs and with the oracle through everything else:
 //     replica state, block tables, leader tables, Instruction streams -- scenario by scenario and over random scripts.
+//     tests/test_sym_abort.py constructs aborts at chosen ticks and CTA positions (the host build logs which site fired,
+//     JR_SYM_ABORT_LOG) and compares, after each launch, the whole table window and the checkpoint bytes as well.
 //
 // Canonical mail (all that can be in flight in a symmetric group):
 //   leader -> each follower, in this order:  [Heartbeat{term, commit}]  [AppendEntries{term, <= 5 blocks}]
@@ -109,6 +111,26 @@ enum : uint32_t {
   SP_ENTER = 10, SP_FILL = 11, SP_LEAVE = 12, SP_TRUNC = 13,   // once per launch: the entry record load, cache fill +
                                                                // encoder init, sym_leave_*, the fused truncation
 };
+// The sites at which a lane aborts (SymGroup::fail).  JR_SYM_ABORT_LOG builds only (the host build of tests/emu,
+// tests/test_sym_abort.py) record, per group and lane, the first site that fired and its tick: d.sab[lane * Gp + g] =
+// site | tick << 8, lane 0 = the leader's side, 1 = the followers' (sym2_kernel: the lane that ran it; sym_kernel: the
+// side the site belongs to).  DESIGN.md §3b lists which test reaches each site.
+enum : uint32_t {
+  SA_FETCH_F = 1,     // followers: fetch_f, a read below flo
+  SA_FIFO_L = 2,      // leader: emit_leader, the raw Instruction FIFO is full
+  SA_FIFO_F = 3,      // followers: emit_followers, the raw Instruction FIFO is full
+  SA_COMMIT = 4,      // leader: leader_commit, the block to commit is missing
+  SA_CLIENT = 5,      // leader: client_request, the id is not above head or falls outside the window
+  SA_HBR = 6,         // leader: leader_tick, HeartbeatResponse{has: false} with a commit above 0
+  SA_EXTEND = 7,      // followers: follower_extend, the parent is missing or the window check fails
+  SA_PROPOSAL = 8,    // leader: the tick loops, a proposal for a follower
+};
+// group s aborts at site `site` (in every other build: exactly the statement `s.abort = true`)
+#ifdef JR_SYM_ABORT_LOG
+#define JR_SYM_ABORT(s, site) ((s).fail(site))
+#else
+#define JR_SYM_ABORT(s, site) ((s).abort = true)
+#endif
 
 // CHECK: the group as sym_check_kernel sees it -- no row caches, every table read goes to global memory.
 template <int R, bool SPLIT = false, bool CHECK = false>
@@ -133,6 +155,17 @@ struct SymGroup {
   uint32_t n_app;                          // most blocks the leader can append in one tick (dense + synthetic proposals)
   bool abort;
   bool share;                              // the followers' Instruction FIFOs are all empty: their records can be shared
+#ifdef JR_SYM_ABORT_LOG
+  uint32_t tick;                           // the tick running now
+  int lane;                                // sym2_kernel: 0 leader lane, 1 follower lane; sym_kernel: -1
+  // leave the canonical evolution at abort site `site` (SA_*, above), and log it (JR_SYM_ABORT)
+  __device__ __forceinline__ void fail(uint32_t site) {
+    const uint32_t side = (site == SA_FETCH_F || site == SA_FIFO_F || site == SA_EXTEND) ? 1u : 0u;
+    uint32_t& e = d.sab[(size_t)(lane < 0 ? side : (uint32_t)lane) * d.Gp + g];
+    if (!abort && !e) e = site | (tick << 8);
+    abort = true;
+  }
+#endif
 #ifdef JR_PROFILE
   long long pt;                            // clock64() at the last phase boundary
   uint32_t prole, pslot;                   // profile role of this lane, phase its cycles go to now
@@ -212,7 +245,7 @@ struct SymGroup {
   // The followers' table, read through the lowest follower's: only rows sym_enter compared across followers (>= flo),
   // rows this launch wrote to all of them, or ids below the floor (absent everywhere) may be answered that way.
   __device__ __forceinline__ void fetch_f(uint32_t bid, uint32_t& next, uint64_t& tok) {
-    if (in_window(bid) && bid < flo) { abort = true; next = ABSENT; tok = 0; return; }
+    if (in_window(bid) && bid < flo) { JR_SYM_ABORT(*this, SA_FETCH_F); next = ABSENT; tok = 0; return; }
     fetch(F0, bid, next, tok);
   }
   __device__ __forceinline__ bool has_f(uint32_t bid) {
@@ -259,7 +292,7 @@ struct SymGroup {
   template <bool NOTIFY>
   __device__ __forceinline__ void emit_leader(uint32_t bid, uint32_t nxa, uint64_t tok) {
     if (!(d.flags & JR_F_CAPTURE_FSM)) return;
-    if (lcnt >= d.Fr) { abort = true; return; }          // step_kernel's raw FIFO would overflow (it drops and counts): its business
+    if (lcnt >= d.Fr) { JR_SYM_ABORT(*this, SA_FIFO_L); return; }       // step_kernel's raw FIFO would overflow (it drops and counts): its business
     const uint32_t outer = phase(NOTIFY ? SP_ENC_NOTIFY : SP_ENC_APPLY);
     if (lcnt + 1u != lwend &&
         run_extend<NOTIFY>(eq(NOTIFY ? 4 : 2), reinterpret_cast<uint2*>(&eq(3))[NOTIFY ? 1 : 0], bid, nxa, tok)) {
@@ -307,7 +340,7 @@ struct SymGroup {
   }
   __device__ __forceinline__ void emit_followers(uint32_t bid, uint32_t next, uint64_t tok) {
     if (!(d.flags & JR_F_CAPTURE_FSM)) return;
-    if (fcnt >= d.Fr) { abort = true; return; }
+    if (fcnt >= d.Fr) { JR_SYM_ABORT(*this, SA_FIFO_F); return; }
     const uint32_t outer = phase(SP_ENC_APPLY);
     if (share && fcnt + 1u != fwend &&
         run_extend<false>(eq(SYM_ENC_L + 1), *reinterpret_cast<uint2*>(&eq(SYM_ENC_L + 2)), bid, next, tok)) {
@@ -367,7 +400,7 @@ struct SymGroup {
     if (above < (uint32_t)(R / 2 + 1)) return;
     const uint32_t q = committed_index(v_new, n_new, v_old);
     if (q <= commit) return;
-    if (!has(L, q)) { abort = true; return; }           // chain.rs:197-202 would panic
+    if (!has(L, q)) { JR_SYM_ABORT(*this, SA_COMMIT); return; }        // chain.rs:197-202 would panic
     const uint32_t prev = commit;
     ckey = 1;
     commit = q;
@@ -383,7 +416,7 @@ struct SymGroup {
   // leader.rs:177-197
   __device__ __forceinline__ void client_request(uint64_t tok) {
     const uint32_t bid = idgen++;
-    if (!(bid > head) || !in_window(bid)) { abort = true; return; }   // chain.rs:163 / engine window: a fault -> step_kernel's business
+    if (!(bid > head) || !in_window(bid)) { JR_SYM_ABORT(*this, SA_CLIENT); return; }   // chain.rs:163 / engine window: a fault -> step_kernel's business
     d.cnext[row(L, bid)] = head;
     d.ctok[row(L, bid)] = tok;
     cache_put(L, bid, head, tok);
@@ -398,7 +431,7 @@ struct SymGroup {
   __device__ __forceinline__ void leader_tick(const SymMail& in, SymMail& out, uint64_t dense_tok, uint32_t n_synth,
                                               uint64_t step_index) {
     // peer mail, ascending sender, FIFO per sender: every follower sent the same [HeartbeatResponse][AppendResponse]
-    if (in.hbr && !in.hbr_has && in.hbr_commit > 0) { abort = true; return; }   // leader.rs:222-231 would replicate mid-drain
+    if (in.hbr && !in.hbr_has && in.hbr_commit > 0) { JR_SYM_ABORT(*this, SA_HBR); return; }   // leader.rs:222-231 would replicate mid-drain
     if (in.ar) {
       phase(SP_AR);
       const uint32_t old = ph_f, v = in.ar_head;
@@ -474,7 +507,7 @@ struct SymGroup {
   // one block of an AppendEntries, applied by every follower (follower.rs:156-173 -> chain.rs:180-190)
   __device__ __forceinline__ void follower_extend(uint32_t bid, uint32_t nx, uint64_t tk) {
     const uint32_t outer = phase(SP_EXTEND);
-    if (nx == ABSENT || !has_f(nx) || !in_window(bid)) { abort = true; return; }   // chain.rs:180-185 Err / window: step_kernel's business
+    if (nx == ABSENT || !has_f(nx) || !in_window(bid)) { JR_SYM_ABORT(*this, SA_EXTEND); return; }   // chain.rs:180-185 Err / window: step_kernel's business
 #pragma unroll
     for (int r = 0; r < R; ++r)
       if ((uint32_t)r != L) {
@@ -982,6 +1015,10 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
   s.last_hb = 0;
   s.share = false;
   s.n_app = 1u + p.n_synth;
+#ifdef JR_SYM_ABORT_LOG
+  s.lane = -1;
+  s.tick = 0;
+#endif
   __shared__ uint4 lane_smem[SYM_SMEM_UNITS * SYM_LANES];
   s.rows = lane_smem + threadIdx.x;
   s.enc = lane_smem + 2 * SYM_ROWS * SYM_LANES + threadIdx.x;
@@ -996,6 +1033,9 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
     const jr_proposal* props = p.proposals;
     s.now = p.now;
     for (uint32_t t = 0; t < p.n_ticks && !s.abort; ++t) {
+#ifdef JR_SYM_ABORT_LOG
+      s.tick = t;
+#endif
       b = SymMail{};
       uint64_t tok = 0;
       if ((p.phases & PH_PROPOSE) && (props || p.tok_runs)) {
@@ -1010,7 +1050,7 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
           props += p.prop_stride;
         }
         if (pr.z == s.L + 1) tok = (uint64_t)pr.x | ((uint64_t)pr.y << 32);
-        else if (pr.z != 0) s.abort = true;               // a proposal for a follower: proxied ClientRequest, not canonical
+        else if (pr.z != 0) JR_SYM_ABORT(s, SA_PROPOSAL);          // a proposal for a follower: proxied ClientRequest, not canonical
       }
       if (s.abort) break;
       s.leader_tick(a, b, tok, (p.phases & PH_PROPOSE) ? p.n_synth : 0u, p.step_index + t);
@@ -1065,6 +1105,10 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.n_app = 1u + p.n_synth;
   s.rows = smem + gi;
   s.enc = smem + 2 * SYM_ROWS * S + gi;
+#ifdef JR_SYM_ABORT_LOG
+  s.lane = lead ? 0 : 1;
+  s.tick = 0;
+#endif
   uint4* mail = smem + SYM_SMEM_UNITS * S + gi;            // [k * S]: k = 2 * buf + {0, 1} leader -> followers, 4 + buf followers -> leader
 #ifdef JR_PROFILE
   for (uint32_t i = threadIdx.x; i < 8 * 3 * 16 * 2; i += blockDim.x) jr_prof_smem()[i] = 0;
@@ -1097,6 +1141,9 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.now = p.now;
   uint32_t cur = 0;                                        // mail buffer written this tick; 1 - cur is read
   for (uint32_t t = 0; t < p.n_ticks; ++t) {
+#ifdef JR_SYM_ABORT_LOG
+    s.tick = t;
+#endif
     s.phase(SP_MAIL_IN);
     if (lead && (JR_SYM2_ROLES & 1)) {
       if (!dead) {
@@ -1118,7 +1165,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
               pr = __ldg(reinterpret_cast<const uint4*>(props + (size_t)t * p.prop_stride) + g);
             }
             if (pr.z == s.L + 1) tok = (uint64_t)pr.x | ((uint64_t)pr.y << 32);
-            else if (pr.z != 0) s.abort = true;           // a proposal for a follower: proxied ClientRequest, not canonical
+            else if (pr.z != 0) JR_SYM_ABORT(s, SA_PROPOSAL);      // a proposal for a follower: proxied ClientRequest, not canonical
           }
           if (!s.abort) s.leader_tick(in, out, tok, (p.phases & PH_PROPOSE) ? p.n_synth : 0u, p.step_index + t);
           if (s.abort) dead = true;

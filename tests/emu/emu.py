@@ -26,6 +26,8 @@ def load() -> C.CDLL:
         lib.jr_engine_destroy.argtypes = [C.c_void_p]
         lib.jr_engine_destroy.restype = None
         lib.jr_last_error.restype = C.c_char_p
+        lib.jr_sym_abort_read.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.c_size_t]
+        lib.jr_sym_abort_read.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -42,3 +44,11 @@ class EmuEngine(RaftApi):
     @classmethod
     def create(cls, n_groups: int, n_replicas: int, **kw) -> "EmuEngine":
         return cls(abi.default_config(n_groups, n_replicas, **kw))
+
+    def sym_aborts(self) -> dict:
+        """jr_sym_abort_read (this build only): {(group, lane): (site, tick)} of the fold's first abort per lane since the
+        last call, lane 0 = the leader's side, 1 = the followers'; site is one of SA_* in sym_fold.cuh.  Clears the log."""
+        G = self.n_groups
+        buf = (C.c_uint32 * (2 * G))()
+        self._check(self._lib.jr_sym_abort_read(self._h, buf, C.c_size_t(2 * G)), "sym_abort_read")
+        return {(i % G, i // G): (v & 255, v >> 8) for i, v in enumerate(buf) if v}
