@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(32 * R, step_min_ctas(R)) step_kernel(const De
       __syncthreads();
     }
   }
-  if (p0.symblk && p0.symblk[blk]) {   // every group of this block was folded by sym_kernel: only keep the hand-over chain alive
+  if (p0.symblk && p0.symblk[blk]) {   // every group of this block was folded by sym2_kernel: only keep the hand-over chain alive
     if (p0.n_parts > 1 && part + 1 < p0.n_parts && threadIdx.x == 0) st_release_u32(d.done + blk, p0.epoch + part + 1);
     return;
   }
@@ -822,7 +822,6 @@ constexpr uint32_t SCAN_THREADS = 1024;
 struct FsmHeader {          // written by fsm_pack_kernel next to the records
   unsigned long long n_records, n_dropped, n_instructions;
   uint32_t node_offset[JR_MAX_REPLICAS + 1];
-  uint32_t ready;           // epoch of the batch, written last
   unsigned long long n_wanted;   // records the FIFOs held, before the cut at the batch's capacity
 };
 
@@ -1186,19 +1185,6 @@ __global__ void fsm_respond_kernel(const Dev d, const RespPlanes q, const FsmHea
   q.rd[i] = drop;
 }
 
-// Packed batch (device) -> the engine's pinned host buffer, by the SMs: the size is only known on the device, so
-// a cudaMemcpyAsync would need a host round trip first.  Runs on the copy-out stream next to the following step.
-__global__ void fsm_copy_kernel(const uint4* __restrict__ src, const FsmHeader* __restrict__ hdr, uint4* __restrict__ dst,
-                                FsmHeader* hdr_dst, uint32_t epoch) {
-  const size_t n = (size_t)hdr->n_records * 2;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = src[i];
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    FsmHeader h = *hdr;
-    h.ready = epoch;
-    *hdr_dst = h;
-  }
-}
-
 __global__ void max_u32_kernel(const uint32_t* v, size_t n, uint32_t* out) {
   uint32_t m = 0;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
@@ -1283,7 +1269,7 @@ struct jr_engine {
   void* verify_buf = nullptr;
   size_t verify_cap = 0;
   // Instruction-stream drain (JR_F_CAPTURE_FSM): scan -> pack into stage[b] on the engine stream, then
-  // fsm_copy_kernel moves stage[b] into the pinned host buffer host[b] on the d2h stream.
+  // the copy engine moves stage[b] into the pinned host buffer host[b] on the d2h stream.
   // One slot more than batches may be outstanding, used round robin: with NBUF batches outstanding at a
   // jr_fsm_records_wait, the next enqueue goes to the spare slot, so the batch just returned is reused no earlier
   // than the second enqueue after the wait (the lifetime the ABI header promises), and never while its take runs.
@@ -1298,12 +1284,10 @@ struct jr_engine {
   cudaEvent_t fsm_landed[NSLOT] = {};                         // copy into host[b] finished (d2h stream)
   size_t fsm_copied[NSLOT] = {};                              // records of stage[b] the enqueued copy covers
   size_t fsm_last_records = 0;                                // size of the last batch taken (the next copy's guess)
-  int fsm_copy_by_sm = 0;                                     // JR_FSM_COPY=sm (A/B): fsm_copy_kernel instead of the copy engine
   bool fsm_used[NSLOT] = {};
   int fsm_i = 0, fsm_pending[NBUF] = {0, 0}, fsm_npending = 0;   // at most NBUF batches outstanding
   std::mutex qmu;   // the two FIFOs of outstanding copy-outs (fsm_pending, tab_pending) and fsm_last_records: a second host thread may
                     // sit in jr_fsm_records_wait / jr_leader_table_wait while the first one keeps submitting
-  uint32_t fsm_epoch = 0;
   // client responses (JR_F_CLIENT_RESPONSES): packed into the second region of stage[b] / host[b] (resp_cap records from
   // record fsm_cap on) with their header at fsm_stage_hdr[b][1] / fsm_host_hdr[b][1]
   RespPlanes rp = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -1318,8 +1302,6 @@ struct jr_engine {
   bool auto_trunc = false;      // jr_set_auto_truncate
   uint32_t auto_trunc_margin = 0;
   int no_fold = 0;              // JR_NO_FOLD=1 (A/B, tests)
-  int no_parts_hint = 0;        // JR_NO_PARTS_HINT=1 (A/B): always cut step_kernel's grid in parts, even while the fold takes every group
-  int sym_one_lane = 0;         // JR_SYM_ONE_LANE=1 (A/B, tests): sym_kernel (one lane per group) instead of sym2_kernel
   uint64_t launches_folded = 0;
   bool last_launch_folded = false;
 };
@@ -1421,11 +1403,8 @@ static void launch_sym_r(jr_engine* e, const StepParams& p) {
     // the entry checks, then the fold that consumes their records: nothing may run between the two
     JR_LAUNCH(sym_check_kernel<R>, (e->d.Gp + SYM_CHECK_THREADS - 1) / SYM_CHECK_THREADS, SYM_CHECK_THREADS, e->stream, e->d, p,
               e->symrec);
-    if (e->sym_one_lane)
-      JR_LAUNCH(sym_kernel<R>, (e->d.Gp + SYM_LANES - 1) / SYM_LANES, SYM_LANES, e->stream, e->d, p, e->symdone, e->symrec);
-    else
-      JR_LAUNCH_SMEM(sym2_kernel<R>, (e->d.Gp + SYM2_GROUPS - 1) / SYM2_GROUPS, 2 * SYM2_GROUPS,
-                     (size_t)SYM2_UNITS * SYM2_GROUPS * sizeof(uint4), e->stream, e->d, p, e->symdone, e->symblk, e->symrec);
+    JR_LAUNCH_SMEM(sym2_kernel<R>, (e->d.Gp + SYM2_GROUPS - 1) / SYM2_GROUPS, 2 * SYM2_GROUPS,
+                   (size_t)SYM2_UNITS * SYM2_GROUPS * sizeof(uint4), e->stream, e->d, p, e->symdone, e->symblk, e->symrec);
   }
 }
 
@@ -1448,10 +1427,6 @@ static jr_status launch_step_once(jr_engine* e, const StepParams& p_in) {
   if (fold_eligible(e, p)) {
     DISPATCH_R(e->cfg.n_replicas, (launch_sym_r<RR>(e, p)));
     CK(cudaGetLastError());
-    if (e->sym_one_lane) {   // (sym2_kernel writes symblk itself)
-      JR_LAUNCH(sym_blocks_kernel, (n_blocks + 127) / 128, 128, e->stream, e->symdone, e->symblk, n_blocks);
-      CK(cudaGetLastError());
-    }
     p.symdone = e->symdone;
     p.symblk = e->symblk;
     e->launches_folded += 1;
@@ -1461,8 +1436,8 @@ static jr_status launch_step_once(jr_engine* e, const StepParams& p_in) {
   // When the fold has been taking every group (no launch of the last two left one behind -- a hint the kernel stores in
   // mapped host memory), step_kernel's CTAs only look at symblk and return: do not cut them in parts, which would cost
   // each of them a ticket and two barriers first.  A wrong guess costs balance in that one launch, nothing else.
-  if (p.symdone && !e->sym_one_lane && e->h_unfolded && (*e->h_unfolded == 0 || p.epoch - *e->h_unfolded > 2u * 8u) && !e->force_parts)
-    if (!e->no_parts_hint) p.n_parts = 1;
+  if (p.symdone && e->h_unfolded && (*e->h_unfolded == 0 || p.epoch - *e->h_unfolded > 2u * 8u) && !e->force_parts)
+    p.n_parts = 1;
   p.part_ticks = (p.n_ticks + p.n_parts - 1) / p.n_parts;
   p.n_parts = (p.n_ticks + p.part_ticks - 1) / p.part_ticks;  // no empty trailing part
   p.n_blocks = n_blocks;
@@ -1475,8 +1450,7 @@ static jr_status launch_step_once(jr_engine* e, const StepParams& p_in) {
   DISPATCH_R(e->cfg.n_replicas, (launch_step_r<RR>(e, p, sorted, grid, smem)));
   CK(cudaGetLastError());
   if (p.trunc) {   // sym2_kernel truncated the groups it folded
-    JR_LAUNCH(truncate_kernel, (e->d.Gp + 127) / 128, 128, e->stream, e->d, p.trunc_margin,
-              (const uint8_t*)((p.symdone && !e->sym_one_lane) ? p.symdone : nullptr));
+    JR_LAUNCH(truncate_kernel, (e->d.Gp + 127) / 128, 128, e->stream, e->d, p.trunc_margin, (const uint8_t*)p.symdone);
     CK(cudaGetLastError());
   }
   e->launches_sorted += sorted ? 1 : 0;
@@ -1665,9 +1639,6 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
     if (aerr == cudaSuccess) *e->h_unfolded = 0;
     if (aerr == cudaSuccess) aerr = cudaHostGetDevicePointer((void**)&e->d.hunf, (void*)e->h_unfolded, 0);
     if (const char* ev = getenv("JR_NO_FOLD")) e->no_fold = atoi(ev);
-    if (const char* ev = getenv("JR_SYM_ONE_LANE")) e->sym_one_lane = atoi(ev);
-    if (const char* ev = getenv("JR_NO_PARTS_HINT")) e->no_parts_hint = atoi(ev);
-    if (const char* ev = getenv("JR_FSM_COPY")) e->fsm_copy_by_sm = strcmp(ev, "sm") == 0;
     if (const char* ev = getenv("JR_PARTS")) e->force_parts = (uint32_t)std::min(std::max(atoi(ev), 0), 8);
 #ifndef JR_EMU
     if (aerr == cudaSuccess) {
@@ -1891,7 +1862,6 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
   e->fsm_i = (b + 1) % jr_engine::NSLOT;
   const size_t plane = (size_t)d.R * d.Gp;
   if (e->fsm_used[b]) CK(cudaStreamWaitEvent(e->stream, e->fsm_landed[b], 0));  // stage[b] has left the device
-  const uint32_t epoch = ++e->fsm_epoch;
 #ifdef JR_EMU
   const uint32_t T = 1, Ts = 1;
 #else
@@ -1921,31 +1891,19 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
   }
   CK(cudaEventRecord(e->fsm_packed[b], e->stream));
   CK(cudaStreamWaitEvent(e->d2h, e->fsm_packed[b], 0));
-  if (e->fsm_copy_by_sm) {
-    JR_LAUNCH(fsm_copy_kernel, 32, 256, e->d2h, e->fsm_stage[b], e->fsm_stage_hdr[b], e->fsm_host[b], e->fsm_host_hdr[b], epoch);
-    CK(cudaGetLastError());
-    e->fsm_copied[b] = e->fsm_cap;
-    if (e->resp_cap) {
-      JR_LAUNCH(fsm_copy_kernel, 32, 256, e->d2h, resp_stage, e->fsm_stage_hdr[b] + 1, e->fsm_host[b] + 2 * (size_t)e->fsm_cap,
-                e->fsm_host_hdr[b] + 1, epoch);
-      CK(cudaGetLastError());
-      e->resp_copied[b] = e->resp_cap;
-    }
-  } else {
-    // Copy engine, speculatively: the batch size is only known on the device, so copy as many records as the previous
-    // batch held plus a margin; fsm_records_take fetches the rest in the (rare) case the batch turned out larger.
-    // (fsm_copy_kernel's stores to host memory share LSUs with the next step's kernel: every SM runs equal
-    // CTAs, so the slowest SM sets its duration.  A DMA copy takes nothing from the SMs.)
-    const size_t guess = std::min<size_t>(e->fsm_cap, std::max<size_t>(last_records + last_records / 8 + 1024, 16384));
-    if (guess) CK(cudaMemcpyAsync(e->fsm_host[b], e->fsm_stage[b], guess * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
-    CK(cudaMemcpyAsync(e->fsm_host_hdr[b], e->fsm_stage_hdr[b], sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
-    e->fsm_copied[b] = guess;
-    if (e->resp_cap) {   // the same scheme for the responses
-      const size_t rg = std::min<size_t>(e->resp_cap, std::max<size_t>(last_resp + last_resp / 8 + 1024, 16384));
-      CK(cudaMemcpyAsync(e->fsm_host[b] + 2 * (size_t)e->fsm_cap, resp_stage, rg * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
-      CK(cudaMemcpyAsync(e->fsm_host_hdr[b] + 1, e->fsm_stage_hdr[b] + 1, sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
-      e->resp_copied[b] = rg;
-    }
+  // Copy engine, speculatively: the batch size is only known on the device, so copy as many records as the previous
+  // batch held plus a margin; fsm_records_take fetches the rest in the (rare) case the batch turned out larger.
+  // (A copy by the SMs would store to host memory with load/store units the next step's kernel needs: every SM runs
+  // equal CTAs, so the slowest SM sets its duration.  A DMA copy takes nothing from the SMs.)
+  const size_t guess = std::min<size_t>(e->fsm_cap, std::max<size_t>(last_records + last_records / 8 + 1024, 16384));
+  if (guess) CK(cudaMemcpyAsync(e->fsm_host[b], e->fsm_stage[b], guess * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
+  CK(cudaMemcpyAsync(e->fsm_host_hdr[b], e->fsm_stage_hdr[b], sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
+  e->fsm_copied[b] = guess;
+  if (e->resp_cap) {   // the same scheme for the responses
+    const size_t rg = std::min<size_t>(e->resp_cap, std::max<size_t>(last_resp + last_resp / 8 + 1024, 16384));
+    CK(cudaMemcpyAsync(e->fsm_host[b] + 2 * (size_t)e->fsm_cap, resp_stage, rg * sizeof(jr_fsm_record), cudaMemcpyDeviceToHost, e->d2h));
+    CK(cudaMemcpyAsync(e->fsm_host_hdr[b] + 1, e->fsm_stage_hdr[b] + 1, sizeof(FsmHeader), cudaMemcpyDeviceToHost, e->d2h));
+    e->resp_copied[b] = rg;
   }
   CK(cudaEventRecord(e->fsm_landed[b], e->d2h));
   e->fsm_used[b] = true;

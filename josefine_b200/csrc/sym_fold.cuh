@@ -1,28 +1,26 @@
-// sym_fold.cuh -- the symmetric-group fold: a whole fused launch of a group in TWO lanes (sym2_kernel), or in one
-// (sym_kernel, the first version: A/B and fallback, JR_SYM_ONE_LANE=1).
+// sym_fold.cuh -- the symmetric-group fold: a whole fused launch of a group in two lanes (sym2_kernel).
 //
 // In a healthy group every follower is in the same state: same term, same head and commit, the same mail from the
 // leader in flight, and the leader holds the same progress entry for each of them.  R-1 replicas then make the same
-// decisions on the same data, tick after tick.  These kernels exploit that symmetry exactly, not approximately:
+// decisions on the same data, tick after tick.  The fold exploits that symmetry exactly, not approximately:
 // the leader's state and ONE follower state that stands for all R-1 followers, the mail between them in its canonical
 // shapes (listed below), and the very handlers of raft_device.cuh -- restated here for scalar operands, each citing
 // the same reference lines -- for all n ticks of the launch.  No mailboxes in HBM, no divergence between roles; what
 // is left is the data that really has to move: the proposal tokens in, the block-table rows of every replica and the
 // Instruction stream out.  sym2_kernel runs the two sides in two lanes of two warps (within a tick they only depend on
 // the previous tick's mail), with the mail, the row caches and the Instruction encoders in shared memory and one
-// barrier per tick; sym_kernel runs both in one lane with the mail in registers.
+// barrier per tick.
 //
 // Exactness contract:
-//   * sym_check_kernel, launched right before either of them with nothing in between, FIRST CHECKS that a group is
+//   * sym_check_kernel, launched right before sym2_kernel with nothing in between, FIRST CHECKS that a group is
 //     symmetric, that its followers' tables agree over every id the launch can read, and that its mail in flight has the
 //     canonical shapes (sym_enter), on the planes the fold is about to read; every other group is left to step_kernel
 //     untouched.  The fold takes the verdict and its starting state from the entry record the check leaves behind.
 //   * If anything outside the canonical evolution would happen during the launch (a fault, an election timer that
-//     could fire, a HeartbeatResponse{has_committed: false}, a read below the compared rows, ...) the lane ABORTS (in
-//     sym2_kernel: tells the other lane through the mail, and both check the other's last mail after the last
-//     barrier): it has only written block-table rows and Instruction records beyond the FIFO counters, which
-//     step_kernel writes identically when it re-runs the group from the untouched state planes -- an abort costs time,
-//     never correctness.
+//     could fire, a HeartbeatResponse{has_committed: false}, a read below the compared rows, ...) the lane ABORTS (it
+//     tells the other lane through the mail, and both check the other's last mail after the last barrier): it has only
+//     written block-table rows and Instruction records beyond the FIFO counters, which step_kernel writes identically
+//     when it re-runs the group from the untouched state planes -- an abort costs time, never correctness.
 //   * On success the replicas' state planes, progress planes and the mailboxes of the last tick are written in the
 //     exact unit layout step_kernel produces, and the Instruction streams leave through the same streaming encoder
 //     fsm_flush uses (fsm_enc_push), fed as the Instructions are produced.
@@ -70,10 +68,6 @@ struct SymMail {
 // after the fill at entry no table READ leaves the SM (rows are still written through to HBM).  (A register shift
 // register costs compare/select chains every tick; local-memory arrays were slower still.)
 constexpr uint32_t SYM_ROWS = 8;
-#ifndef JR_SYM_LANES
-#define JR_SYM_LANES 128   // (A/B builds override it)
-#endif
-constexpr uint32_t SYM_LANES = JR_SYM_LANES;   // threads per CTA of sym_kernel: one warp per SM sub-partition
 // The Instruction streams are encoded AS THEY ARE PRODUCED, by the same streaming encoder fsm_flush uses (fsm_enc_push):
 // its state is parked in shared memory between two Instructions, [slot][lane] like the row caches.  (The raw FIFO +
 // fsm_flush round trip of step_kernel cost this kernel a quarter of its instructions and half of its DRAM traffic.)
@@ -84,8 +78,8 @@ constexpr uint32_t SYM_LANES = JR_SYM_LANES;   // threads per CTA of sym_kernel:
 constexpr uint32_t SYM_ENC_L = 5, SYM_ENC_F = 3;
 constexpr uint32_t SYM_SMEM_UNITS = 2 * SYM_ROWS + SYM_ENC_L + SYM_ENC_F;   // uint4 per lane
 // sym2_kernel: TWO lanes per group, in two warps of the same CTA -- one runs the leader's handlers, the other the
-// followers' -- because within a tick the two sides only depend on the mail of the PREVIOUS tick.  The kernel is latency
-// bound with 3.5 warps per SM sub-partition; this doubles the warps and halves each warp's serial chain.  The mail goes
+// followers' -- because within a tick the two sides only depend on the mail of the PREVIOUS tick.  One lane per group is
+// latency bound with 3.5 warps per SM sub-partition; two double the warps and halve each warp's serial chain.  The mail goes
 // through shared memory, double buffered, one __syncthreads() per tick:
 //   leader -> followers   A = {hb | ae << 1 | nb << 4 | abort << 8 | ids << 9 | mode << 10, commit, leader's max key, id0 / progress head}
 //                         B = {id1 .. id4}   (ids = 1: the AppendEntries' blocks are listed -- the mail sym_enter found in
@@ -113,8 +107,7 @@ enum : uint32_t {
 };
 // The sites at which a lane aborts (SymGroup::fail).  JR_SYM_ABORT_LOG builds only (the host build of tests/emu,
 // tests/test_sym_abort.py) record, per group and lane, the first site that fired and its tick: d.sab[lane * Gp + g] =
-// site | tick << 8, lane 0 = the leader's side, 1 = the followers' (sym2_kernel: the lane that ran it; sym_kernel: the
-// side the site belongs to).  DESIGN.md §3b lists which test reaches each site.
+// site | tick << 8, lane 0 = the leader lane, 1 = the follower lane.  DESIGN.md §3b lists which test reaches each site.
 enum : uint32_t {
   SA_FETCH_F = 1,     // followers: fetch_f, a read below flo
   SA_FIFO_L = 2,      // leader: emit_leader, the raw Instruction FIFO is full
@@ -133,9 +126,9 @@ enum : uint32_t {
 #endif
 
 // CHECK: the group as sym_check_kernel sees it -- no row caches, every table read goes to global memory.
-template <int R, bool SPLIT = false, bool CHECK = false>
+template <int R, bool CHECK = false>
 struct SymGroup {
-  static constexpr uint32_t STRIDE = SPLIT ? SYM2_GROUPS : SYM_LANES;   // columns of the CTA's per-group shared memory
+  static constexpr uint32_t STRIDE = SYM2_GROUPS;   // columns of the CTA's per-group shared memory
   const Dev& d;
   const uint32_t g;
   const size_t plane;
@@ -157,11 +150,10 @@ struct SymGroup {
   bool share;                              // the followers' Instruction FIFOs are all empty: their records can be shared
 #ifdef JR_SYM_ABORT_LOG
   uint32_t tick;                           // the tick running now
-  int lane;                                // sym2_kernel: 0 leader lane, 1 follower lane; sym_kernel: -1
+  int lane;                                // 0 leader lane, 1 follower lane
   // leave the canonical evolution at abort site `site` (SA_*, above), and log it (JR_SYM_ABORT)
   __device__ __forceinline__ void fail(uint32_t site) {
-    const uint32_t side = (site == SA_FETCH_F || site == SA_FIFO_F || site == SA_EXTEND) ? 1u : 0u;
-    uint32_t& e = d.sab[(size_t)(lane < 0 ? side : (uint32_t)lane) * d.Gp + g];
+    uint32_t& e = d.sab[(size_t)lane * d.Gp + g];
     if (!abort && !e) e = site | (tick << 8);
     abort = true;
   }
@@ -173,10 +165,8 @@ struct SymGroup {
   // phase it closed, so a nested phase can hand the time back to its caller's
   __device__ __forceinline__ uint32_t phase(uint32_t slot) {
     const uint32_t o = pslot;
-    if constexpr (SPLIT) {   // (sym_kernel is not profiled: its shared memory has no room for the counters)
-      JR_PROF_ADD(prole, o, pt);
-      pslot = slot;
-    }
+    JR_PROF_ADD(prole, o, pt);
+    pslot = slot;
     return o;
   }
 #else
@@ -203,14 +193,12 @@ struct SymGroup {
     if (e.x == bid) { next = e.y; tok = (uint64_t)e.z | ((uint64_t)e.w << 32); return; }
     next = __ldcg(d.cnext + row(r, bid));   // rows written earlier in this launch by this lane: read them at L2
     tok = __ldcg(d.ctok + row(r, bid));
-    if (!SPLIT) cache_put(r, bid, next, tok);   // (split kernel: a cache is only written at entry and by appends, see fetch_sent)
   }
   // sym2_kernel, follower lane: a block the leader sent one tick ago, read from the LEADER's row cache, which the leader
   // lane is appending to right now.  Its appends of this tick are the ids (mk_sent, mk_sent + n_app]; a slot one of them
   // maps to is not read (the row is in global memory, written before the last barrier).  No other write happens to that
-  // cache after entry, so every slot this reads is quiescent.
+  // cache after entry (fetch does not cache a miss), so every slot this reads is quiescent.
   __device__ __forceinline__ void fetch_sent(uint32_t bid, uint32_t mk_sent, uint32_t n_app, uint32_t& next, uint64_t& tok) {
-    if (!SPLIT) { fetch(L, bid, next, tok); return; }
     if (!in_window(bid)) { next = ABSENT; tok = 0; return; }
     if (bid + SYM_ROWS > mk_sent + n_app) {
       const uint4 e = slot(L, bid);
@@ -219,7 +207,7 @@ struct SymGroup {
     next = __ldcg(d.cnext + row(L, bid));
     tok = __ldcg(d.ctok + row(L, bid));
   }
-  __device__ __forceinline__ void cache_clear(uint32_t first = 0, uint32_t n = 2 * SYM_ROWS) const {
+  __device__ __forceinline__ void cache_clear(uint32_t first, uint32_t n) const {
 #pragma unroll
     for (uint32_t k = 0; k < 2 * SYM_ROWS; ++k)
       if (k >= first && k < first + n) rows[k * STRIDE] = make_uint4(ABSENT, ABSENT, 0u, 0u);   // tag ABSENT matches no id
@@ -457,14 +445,12 @@ struct SymGroup {
     }
     out.ae = 1;                                            // replicate() follows: one AppendEntries per peer
     out.mk = maxkey;
-    if (!SPLIT) replicate(ph_f, mode_f, maxkey, out);
   }
   // replicate, leader.rs:124-174: Probe -> range(head..).nth(1); Replicate -> range(head..).skip(1).take(5), over the
-  // leader's table as it stood when its largest key was `mk`.  The one-lane kernel runs it inside the leader's tick.  In
-  // sym2_kernel the FOLLOWER lane runs the same scan at the start of the next tick (follower_tick_view), from the
-  // {progress head, mode, max key} the leader lane put in its mail -- the same rows, read through fetch_sent, the same
-  // blocks; it takes a sixth of the leader's chain off the critical lane.  (The leader lane runs this once itself, for
-  // the outbox the launch leaves behind.)
+  // leader's table as it stood when its largest key was `mk`.  The leader lane runs it once, at exit, for the outbox the
+  // launch leaves behind.  Within the launch the FOLLOWER lane runs the same scan at the start of the next tick
+  // (follower_tick_view), from the {progress head, mode, max key} the leader lane put in its mail -- the same rows, read
+  // through fetch_sent, the same blocks; that takes a sixth of the leader's chain off the critical lane.
   __device__ __forceinline__ void replicate(uint32_t phf, uint32_t modef, uint32_t mk, SymMail& out) {
     const uint32_t take = modef ? JR_MAX_AE_BLOCKS : 1u;
     uint32_t bid = max(phf, tbase), pulled = 0, nb = 0;
@@ -572,7 +558,7 @@ struct SymGroup {
 
 // ---- entry: is the group symmetric, is its mail canonical? (run by sym_check_kernel, below) ---------------------------
 template <int R>
-__device__ __forceinline__ bool sym_enter(SymGroup<R, false, true>& s, SymMail& m, const StepParams& p, int prv) {
+__device__ __forceinline__ bool sym_enter(SymGroup<R, true>& s, SymMail& m, const StepParams& p, int prv) {
   const Dev& d = s.d;
   if (s.g >= d.G) return false;
   // roles: one live leader, R-1 live followers of that leader
@@ -812,7 +798,7 @@ __global__ void __launch_bounds__(SYM_CHECK_THREADS, JR_SYM_CHECK_MINCTAS) sym_c
   if (g >= d.Gp) return;
   const size_t n = d.Gp;
   uint32_t* w = rec + g;
-  SymGroup<R, false, true> s(d, g);
+  SymGroup<R, true> s(d, g);
   SymMail m;
   if (!sym_enter(s, m, p, 1 - p.cur)) { w[SR_FLAGS * n] = 0u; return; }
   const uint32_t L = s.L;
@@ -852,8 +838,8 @@ __global__ void __launch_bounds__(SYM_CHECK_THREADS, JR_SYM_CHECK_MINCTAS) sym_c
 
 // The entry record of group s.g (< Gp), one round of loads: LEAD the leader's side (and fc = its FSM counters), FOLLOW
 // the followers' side.  false: the group does not fold.
-template <bool LEAD, bool FOLLOW, int R, bool SPLIT>
-__device__ __forceinline__ bool sym_load(SymGroup<R, SPLIT>& s, SymMail& m, const uint32_t* rec, uint2& fc) {
+template <bool LEAD, bool FOLLOW, int R>
+__device__ __forceinline__ bool sym_load(SymGroup<R>& s, SymMail& m, const uint32_t* rec, uint2& fc) {
   const uint32_t* w = rec + s.g;
   const size_t n = s.d.Gp;
   const uint32_t f = __ldg(w + SR_FLAGS * n);
@@ -894,8 +880,8 @@ __device__ __forceinline__ bool sym_load(SymGroup<R, SPLIT>& s, SymMail& m, cons
 }
 
 // ---- exit: write everything step_kernel would have left behind -------------------------------------------------------
-template <int R, bool SPLIT>
-__device__ __forceinline__ void sym_leave_leader(SymGroup<R, SPLIT>& s, const SymMail& last, int cur_last, const uint32_t* rec) {
+template <int R>
+__device__ __forceinline__ void sym_leave_leader(SymGroup<R>& s, const SymMail& last, int cur_last, const uint32_t* rec) {
   const Dev& d = s.d;
   const uint32_t L = s.L;
   {  // leader: P2, P3, progress planes, max key (P0 / P1 are untouched by a steady leader)
@@ -950,8 +936,8 @@ __device__ __forceinline__ void sym_leave_leader(SymGroup<R, SPLIT>& s, const Sy
   }
 }
 
-template <int R, bool SPLIT>
-__device__ __forceinline__ void sym_leave_followers(SymGroup<R, SPLIT>& s, const SymMail& last, int cur_last, const uint32_t* rec) {
+template <int R>
+__device__ __forceinline__ void sym_leave_followers(SymGroup<R>& s, const SymMail& last, int cur_last, const uint32_t* rec) {
   const Dev& d = s.d;
   const uint32_t L = s.L;
   // The followers emitted the same Instructions.  If none of them has anything pending since the last drain, ONE set of
@@ -1001,74 +987,6 @@ __device__ __forceinline__ void sym_leave_followers(SymGroup<R, SPLIT>& s, const
   }
 }
 
-// One lane per group.  symdone[g] = 1: the whole launch of group g has been applied here; 0: step_kernel runs it.
-template <int R>
-__global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const Dev d, const StepParams p, uint8_t* symdone,
-                                                                        const uint32_t* rec) {
-  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= d.Gp) return;
-  SymGroup<R> s(d, g);
-  SymMail a, b;
-  s.abort = false;
-  s.lcnt = s.fcnt = 0;
-  s.n_hb = 0;
-  s.last_hb = 0;
-  s.share = false;
-  s.n_app = 1u + p.n_synth;
-#ifdef JR_SYM_ABORT_LOG
-  s.lane = -1;
-  s.tick = 0;
-#endif
-  __shared__ uint4 lane_smem[SYM_SMEM_UNITS * SYM_LANES];
-  s.rows = lane_smem + threadIdx.x;
-  s.enc = lane_smem + 2 * SYM_ROWS * SYM_LANES + threadIdx.x;
-  s.cache_clear();
-  uint2 fcl;
-  bool ok = sym_load<true, true>(s, a, rec, fcl);
-  if (ok) {
-    s.cache_fill(s.L, s.maxkey);
-    s.cache_fill(s.F0, s.fmaxkey);
-    s.enc_init_leader(fcl);
-    s.enc_init_followers();
-    const jr_proposal* props = p.proposals;
-    s.now = p.now;
-    for (uint32_t t = 0; t < p.n_ticks && !s.abort; ++t) {
-#ifdef JR_SYM_ABORT_LOG
-      s.tick = t;
-#endif
-      b = SymMail{};
-      uint64_t tok = 0;
-      if ((p.phases & PH_PROPOSE) && (props || p.tok_runs)) {
-        uint4 pr;
-        if (p.tok_runs) {
-          const uint4 rn = __ldg(p.tok_runs + g);
-          const uint64_t base = (uint64_t)rn.x | ((uint64_t)rn.y << 32);
-          const uint64_t tk = base + (uint64_t)(p.tok_tick + t) * ((uint64_t)rn.z | ((uint64_t)rn.w << 32));
-          pr = make_uint4((uint32_t)tk, (uint32_t)(tk >> 32), base ? __ldg(p.tok_route + g) : 0u, 0u);
-        } else {
-          pr = __ldg(reinterpret_cast<const uint4*>(props) + g);
-          props += p.prop_stride;
-        }
-        if (pr.z == s.L + 1) tok = (uint64_t)pr.x | ((uint64_t)pr.y << 32);
-        else if (pr.z != 0) JR_SYM_ABORT(s, SA_PROPOSAL);          // a proposal for a follower: proxied ClientRequest, not canonical
-      }
-      if (s.abort) break;
-      s.leader_tick(a, b, tok, (p.phases & PH_PROPOSE) ? p.n_synth : 0u, p.step_index + t);
-      if (s.abort) break;
-      s.follower_tick(a, b);
-      a = b;
-      s.now += p.dt;
-    }
-    ok = !s.abort;
-    if (ok) {
-      const int cur_last = p.cur ^ (int)((p.n_ticks - 1) & 1u);
-      sym_leave_leader(s, a, cur_last, rec);
-      sym_leave_followers(s, a, cur_last, rec);
-    }
-  }
-  symdone[g] = ok ? 1 : 0;
-}
-
 // Two lanes per group (see SYM2_GROUPS above).  Both lanes take the same verdict from the group's entry record, each
 // loading the words of its side; afterwards each keeps to its side: the leader lane owns the leader's table cache, encoder state,
 // planes and outbox, the follower lane those of the followers.  Either side may abort: it says so in its mail, the
@@ -1079,9 +997,6 @@ __global__ void __launch_bounds__(SYM_LANES, 512 / SYM_LANES) sym_kernel(const D
 // two waves faster than 7 (72 registers, spilling) run one and a bit.
 #ifndef JR_SYM2_MINCTAS
 #define JR_SYM2_MINCTAS 4
-#endif
-#ifndef JR_SYM2_ROLES
-#define JR_SYM2_ROLES 3   // (register-need experiments: 1 = leader code only, 2 = follower code only)
 #endif
 template <int R>
 __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(const Dev d, const StepParams p, uint8_t* symdone, uint8_t* symblk,
@@ -1096,7 +1011,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   const bool lead = ((w ^ blockIdx.x) & 1u) == 0;          // roles alternate from CTA to CTA: no SM sub-partition gets leaders only
   const uint32_t gi = (w >> 1) * 32u + lane;               // group within the CTA
   const uint32_t g = blockIdx.x * S + gi;                  // (g >= Gp: no record; the lane only keeps the barriers company)
-  SymGroup<R, true> s(d, g);
+  SymGroup<R> s(d, g);
   s.abort = false;
   s.lcnt = s.fcnt = 0;
   s.n_hb = 0;
@@ -1145,7 +1060,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
     s.tick = t;
 #endif
     s.phase(SP_MAIL_IN);
-    if (lead && (JR_SYM2_ROLES & 1)) {
+    if (lead) {
       if (!dead) {
         const uint4 c = mail[(4 + (1 - cur)) * S];
         if (c.x & SYM2_ABORT) dead = true;
@@ -1176,7 +1091,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
         }
       }
       if (dead) mail[(2 * cur) * S] = make_uint4(SYM2_ABORT, 0u, 0u, 0u);
-    } else if (!lead && (JR_SYM2_ROLES & 2)) {
+    } else {
       if (!dead) {
         const uint4 ma = mail[(2 * (1 - cur)) * S];
         if (ma.x & SYM2_ABORT) dead = true;
@@ -1253,16 +1168,6 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
       if (v) atomicAdd(d.prof + (i % (3 * 16 * 2)), v);
     }
 #endif
-}
-
-// symblk[b] = every group of 32-group block b was folded (step_kernel CTAs of such blocks return at once)
-__global__ void sym_blocks_kernel(const uint8_t* symdone, uint8_t* symblk, uint32_t n_blocks) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= n_blocks) return;
-  const uint4* v = reinterpret_cast<const uint4*>(symdone + (size_t)b * GROUPS_PER_CTA);
-  const uint4 x = v[0], y = v[1];
-  const uint32_t all = 0x01010101u;
-  symblk[b] = (x.x == all && x.y == all && x.z == all && x.w == all && y.x == all && y.y == all && y.z == all && y.w == all) ? 1 : 0;
 }
 
 #endif  // JR_DEVICE_CODE

@@ -28,7 +28,7 @@ ABSENT = 0xFFFFFFFF
 CAP = abi.F_CAPTURE_FSM
 HB, DT, SPREAD = 250, 100, 8        # heartbeat, tick; group g's leader is g % SPREAD ids behind the top at the shift
 CFG = dict(chain_capacity=100, heartbeat_ms=HB, mailbox_units=64, fsm_units=256)     # rows = 128
-KINDS = ("fold", "nofold", "one_lane", "responses")
+KINDS = ("fold", "nofold", "responses")
 
 
 def _oracle(g, r, **kw):
@@ -47,9 +47,9 @@ def _gpu(g, r, **kw):
 
 
 def _create(make, kind, G, R, monkeypatch, **cfg):
-    """fold: folds; nofold: JR_NO_FOLD=1 and stream digests; one_lane: JR_SYM_ONE_LANE=1; responses: F_CLIENT_RESPONSES."""
+    """fold: folds; nofold: JR_NO_FOLD=1 and stream digests; responses: F_CLIENT_RESPONSES."""
     flags = CAP | {"nofold": abi.F_STREAM_DIGEST, "responses": abi.F_CLIENT_RESPONSES}.get(kind, 0)
-    env = {"nofold": "JR_NO_FOLD", "one_lane": "JR_SYM_ONE_LANE"}.get(kind)
+    env = {"nofold": "JR_NO_FOLD"}.get(kind)
     if env:
         monkeypatch.setenv(env, "1")
     api = make(G, R, flags=flags, **cfg)

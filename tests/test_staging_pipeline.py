@@ -4,8 +4,7 @@ jr_leader_table_wait + jr_fsm_records_wait (+ jr_fsm_responses), on the submitti
 
 Every consumed batch is compared with the C++ oracle making the same calls in the same program order: its synchronous
 leader_table where the engine calls jr_leader_table_async (routing is stream-ordered), its drain_fsm where the engine
-enqueues the batch.  Runs on the device code built for the host (tests/emu) and on the GPU, over both copy paths of the
-drain: the copy engine with its speculative size guess (default) and fsm_copy_kernel (JR_FSM_COPY=sm)."""
+enqueues the batch.  Runs on the device code built for the host (tests/emu) and on the GPU."""
 import ctypes as C
 import os
 import threading
@@ -272,17 +271,6 @@ def drive(p, plan, before=None):
         p.check(p.read(t))
 
 
-def _copy_params():
-    return [pytest.param("dma", id="dma"), pytest.param("sm", id="sm")]
-
-
-def _set_copy(monkeypatch, copy):
-    if copy == "sm":
-        monkeypatch.setenv("JR_FSM_COPY", "sm")
-    else:
-        monkeypatch.delenv("JR_FSM_COPY", raising=False)
-
-
 def _where():
     return [pytest.param(_emu, id="emu"), pytest.param(_gpu, id="gpu", marks=pytest.mark.gpu)]
 
@@ -291,13 +279,11 @@ def _where():
 
 @pytest.mark.parametrize("resp", [False, True], ids=["records", "responses"])
 @pytest.mark.parametrize("depth", [1, 2, 3])
-@pytest.mark.parametrize("copy", _copy_params())
 @pytest.mark.parametrize("make", _where())
-def test_returned_batch_survives_the_next_enqueue(make, copy, depth, resp, monkeypatch):
+def test_returned_batch_survives_the_next_enqueue(make, depth, resp):
     """The header: the records (and responses) jr_fsm_records_wait returns stay valid until the JR_STAGING_DEPTH-1'th
     jr_fsm_records_async after it.  With `depth` batches outstanding at the wait, one more quantum and its enqueue must
     leave the returned bytes untouched, and they must be the oracle's drain of that quantum."""
-    _set_copy(monkeypatch, copy)
     G, R, S = 8, 3, 8
     p = Pipeline(make, G, R, S, api="tokens", resp=resp, chain_capacity=256, fsm_units=64)
     try:
@@ -346,9 +332,7 @@ def _loop_plan(G, S, n=8):
 @pytest.mark.parametrize("api,resp", [("token_runs", True), ("tokens", False)])
 @pytest.mark.parametrize("R", [3, 5])
 @pytest.mark.parametrize("G", [33, 96])
-@pytest.mark.parametrize("copy", _copy_params())
-def test_pipelined_loop_on_device_code(copy, G, R, api, resp, monkeypatch):
-    _set_copy(monkeypatch, copy)
+def test_pipelined_loop_on_device_code(G, R, api, resp):
     S = 16
     p = Pipeline(_emu, G, R, S, api=api, resp=resp, seed=G + R, chain_capacity=256, fsm_units=4 * S + 64)
     try:
@@ -361,11 +345,9 @@ def test_pipelined_loop_on_device_code(copy, G, R, api, resp, monkeypatch):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("G,api,copy", [(4096, "token_runs", "dma"), (4096, "token_runs", "sm"), (4096, "tokens", "dma"),
-                                        (4096, "tokens", "sm"), (65536, "token_runs", "dma"), (65536, "tokens", "sm")])
-def test_pipelined_loop_on_gpu(G, api, copy, monkeypatch):
+@pytest.mark.parametrize("G,api", [(4096, "token_runs"), (4096, "tokens"), (65536, "token_runs")])
+def test_pipelined_loop_on_gpu(G, api):
     """4,096 x 5 and 65,536 x 5, 64-tick quanta: batches of 4,096 records and more, so jr_fsm_fold_mt folds on threads."""
-    _set_copy(monkeypatch, copy)
     R, S = 5, 64
     p = Pipeline(_gpu, G, R, S, api=api, seed=3, chain_capacity=512, fsm_units=2 * S + 32, fsm_host_records=4 * G * R)
     try:
@@ -393,13 +375,11 @@ def _tail_plan(G, S, n, at, seed):
     return plan
 
 
-@pytest.mark.parametrize("copy", _copy_params())
 @pytest.mark.parametrize("make", _where())
-def test_batch_larger_than_the_copy_guess(make, copy, monkeypatch):
+def test_batch_larger_than_the_copy_guess(make):
     """After constant-stride quanta (a few records per replica), a quantum of arbitrary tokens (no constant stride to
     run-length encode) with two other batches outstanding: its batch outgrows the speculative copy, whose tail
     fsm_records_take fetches -- the batch must still be the oracle's."""
-    _set_copy(monkeypatch, copy)
     G, R, S, AT = 384, 5, 48, 4          # ~1.5 records per group-tick of arbitrary tokens: ~27,000 records > 16,384
     p = Pipeline(make, G, R, S, api="token_runs", resp=True, seed=9, chain_capacity=256, fsm_units=4 * S + 64,
                  fsm_host_records=G * (R + 1) * S + 4096)
@@ -415,13 +395,11 @@ def test_batch_larger_than_the_copy_guess(make, copy, monkeypatch):
 # ---- (d) two host threads ----------------------------------------------------------------------------------------------
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("copy", _copy_params())
-def test_consumer_thread_on_gpu(copy, monkeypatch):
+def test_consumer_thread_on_gpu():
     """A consumer thread waits for, expands, folds and reads the responses of quantum k while the submitting thread
     enqueues quantum k+3: the header lets the submitter go on as soon as k's wait has returned, and asks only that the
     consumer be done with k before the submitter's second enqueue after that wait (k+4).  Includes a quantum that
     outgrows the speculative copy.  Every batch is checked against the oracle afterwards, over the same call log."""
-    _set_copy(monkeypatch, copy)
     G, R, S, N, AT = 4096, 5, 32, 10, 5
     p = Pipeline(_gpu, G, R, S, api="token_runs", resp=True, seed=5, chain_capacity=512, fsm_units=4 * S + 64,
                  fsm_host_records=G * (R + 1) * S + 4096)

@@ -1,7 +1,7 @@
-"""The fold's mid-launch fallback (josefine_b200/csrc/sym_fold.cuh, DESIGN.md §3b): a lane of sym2_kernel / sym_kernel
-that meets anything outside the canonical evolution aborts, the group is handed back to step_kernel, and the abort must
-cost time, never correctness.  Here the aborts are constructed -- at a chosen tick, on a chosen lane, at chosen
-positions in the CTAs of both kernels -- and after every launch the folding engine must equal the never-folding engine
+"""The fold's mid-launch fallback (josefine_b200/csrc/sym_fold.cuh, DESIGN.md §3b): a lane of sym2_kernel that meets
+anything outside the canonical evolution aborts, the group is handed back to step_kernel, and the abort must cost time,
+never correctness.  Here the aborts are constructed -- at a chosen tick, on a chosen lane, at chosen positions in the
+CTAs of sym2_kernel and step_kernel -- and after every launch the folding engine must equal the never-folding engine
 and the oracle on everything: the Instruction stream, replica states, leader tables, the whole block-table window of
 every replica around the aborted groups (ids above every head included), and the checkpoint bytes segment by segment
 (the only place the outboxes, the progress planes and the queues are compared exactly).
@@ -246,11 +246,6 @@ def case_proposal_aborts(make, G, R, lead=1, n=9, rounds=2, every=1, cfg_over=No
 @pytest.mark.parametrize("R,lead", [(2, 1), (3, 2), (5, 1), (5, 4), (8, 3)])
 def test_proposal_aborts_on_device_code(R, lead):
     case_proposal_aborts(_emu, 150 if R <= 5 else 72, R, lead=lead)
-
-
-def test_proposal_aborts_one_lane_kernel_on_device_code(monkeypatch):
-    monkeypatch.setenv("JR_SYM_ONE_LANE", "1")
-    case_proposal_aborts(_emu, 150, 3, lead=2)
 
 
 def test_proposal_aborts_split_launches_on_device_code(monkeypatch):

@@ -168,16 +168,10 @@ def _gpu(g, r, **kw):
     return RaftEngine.create(g, r, **kw)
 
 
-@pytest.mark.parametrize("one_lane", [False, True])
-def test_entry_checks_on_device_code(one_lane, monkeypatch):
-    if one_lane:
-        monkeypatch.setenv("JR_SYM_ONE_LANE", "1")
+def test_entry_checks_on_device_code(monkeypatch):
     case_entry_checks(_emu, monkeypatch)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("one_lane", [False, True])
-def test_entry_checks_on_gpu(one_lane, monkeypatch):
-    if one_lane:
-        monkeypatch.setenv("JR_SYM_ONE_LANE", "1")
+def test_entry_checks_on_gpu(monkeypatch):
     case_entry_checks(_gpu, monkeypatch)
