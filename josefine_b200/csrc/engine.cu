@@ -7,6 +7,7 @@
 // replica state machine is in raft_device.cuh.
 #include <algorithm>
 #include <atomic>
+#include <cassert>
 #include <chrono>
 #include <cstdarg>
 #include <cstdio>
@@ -113,8 +114,8 @@ __global__ void __launch_bounds__(32 * R, step_min_ctas(R)) step_kernel(const De
     uint32_t lead = R;
 #pragma unroll
     for (int rr = 0; rr < R; ++rr) {
-      const uint32_t m = d.p2[(size_t)rr * d.Gp + g].w;
-      if (lead == (uint32_t)R && (m & 255u) == JR_ROLE_LEADER && ((m >> 8) & 255u) == 0 && !((m >> 27) & 1u)) lead = rr;
+      const uint32_t m = d.p2[(size_t)rr * d.Gp + g].w, role = meta_role(m), fault = meta_fault(m), dead = meta_dead(m);
+      if (lead == (uint32_t)R && role == JR_ROLE_LEADER && fault == 0 && !dead) lead = rr;
     }
     if (lead != (uint32_t)R) r = w == 0 ? lead : (w <= lead ? w - 1 : w);
   }
@@ -231,7 +232,7 @@ __global__ void init_kernel(const Dev d) {
   d.p0[i] = make_uint4(0, 0, 0, 0);
   d.p1[i] = make_uint4(0, 0, timeout, 1);                 // init(): first draw, election_time = 0
   // head 0, commit 0, id_gen 1; a node this engine does not host is inert (the `dead` bit)
-  d.p2[i] = make_uint4(0, 0, 1, JR_ROLE_FOLLOWER | (((d.resident >> r) & 1u) ? 0u : (1u << 27)));
+  d.p2[i] = make_uint4(0, 0, 1, meta_pack(JR_ROLE_FOLLOWER, 0, 0, 0, ((d.resident >> r) & 1u) ? 0u : 1u, 0));
   d.p3[i] = make_uint4(0, 0, 0, 0);
   d.mk[i] = 0;
   d.cnext[i] = 0;                                         // genesis block 0 -> 0 (chain.rs:139-153)
@@ -251,50 +252,95 @@ __global__ void compact_kernel(const Dev d) {
   const size_t plane = (size_t)d.R * d.Gp;
   if (i >= plane || (uint32_t)(i % d.Gp) >= d.G) return;
   const uint4 c = d.p2[i];
-  const uint32_t meta = c.w;
-  if (((meta >> 8) & 255u) != 0 || ((meta >> 27) & 1u)) return;  // faulted or dead
+  if (!meta_live(c.w)) return;  // faulted or dead
   bool have = false;
   uint32_t expect = 0;
   const uint32_t floor = d.tb[i % d.Gp];
   for (uint32_t b = c.y; b-- > floor;) {  // ids in [0, commit), descending; nothing is left below the floor (D7)
     if (b - floor >= d.cap) continue;    // (a commit past the window cannot exist: chain_commit needs the block)
-    const uint32_t nx = d.cnext[(size_t)(b & d.capm) * plane + i];
+    const uint32_t nx = d.cnext[table_row(d, plane, b, i)];
     if (nx == ABSENT) continue;
-    if (have && b != expect) d.cnext[(size_t)(b & d.capm) * plane + i] = ABSENT;
+    if (have && b != expect) d.cnext[table_row(d, plane, b, i)] = ABSENT;
     expect = nx;  // even for a removed block
     have = true;
   }
 }
 
-// Adds every thread's v into *out (one atomic per CTA on the device).
-__device__ inline void block_add(unsigned long long* out, uint64_t v, uint64_t* smem) {
+// ---- CTA-wide sum and exclusive scan ------------------------------------------------------------------------------
+// The kernels built on these run CTAs of CTA_THREADS threads (fsm_scan_kernel: one CTA of SCAN_THREADS), multiples of 32.
+// The CPU emulation (tests/emu) runs a CTA's threads one after another, with no warp shuffles and no barriers, so there
+// these kernels run one-thread CTAs, where both primitives are the identity.
 #ifdef JR_EMU
-  (void)smem;
-  atomicAdd(out, (unsigned long long)v);
+constexpr uint32_t CTA_THREADS = 1, SCAN_THREADS = 1;
 #else
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    uint64_t t = threadIdx.x < (blockDim.x >> 5) ? smem[threadIdx.x] : 0;
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_down_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0) atomicAdd(out, (unsigned long long)t);
+constexpr uint32_t CTA_THREADS = 256, SCAN_THREADS = 1024;
+#endif
+
+struct SumOp { template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return a + b; } };
+struct MaxOp { template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return max(a, b); } };
+
+// Combines each of the N values over the CTA's threads; thread 0 ends with the CTA totals in v.  smem: one word per
+// value and warp; it may be reused after a __syncthreads().
+template <class T, int N, class Op = SumOp>
+__device__ __forceinline__ void cta_sum(T (&v)[N], T (&smem)[N][32], Op op = Op()) {
+#ifdef JR_EMU
+  assert(blockDim.x == 1);
+  (void)smem; (void)op;
+#else
+  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int c = 0; c < N; ++c) {
+    for (int o = 16; o > 0; o >>= 1) v[c] = op(v[c], __shfl_down_sync(0xffffffffu, v[c], o));
+    if (lane == 0) smem[c][w] = v[c];
   }
   __syncthreads();
+  if (threadIdx.x == 0)
+    for (uint32_t k = 1; k < (blockDim.x + 31) / 32; ++k)
+#pragma unroll
+      for (int c = 0; c < N; ++c) v[c] = op(v[c], smem[c][k]);
+#endif
+}
+
+// Returns the sum of v over the CTA's threads below this one; *total (if given) = the sum over all of them.  smem: one
+// word per warp; it may be reused after a __syncthreads().
+template <class T>
+__device__ __forceinline__ T cta_exclusive_scan(T v, T* smem, T* total = nullptr) {
+#ifdef JR_EMU
+  assert(blockDim.x == 1);
+  (void)smem;
+  if (total) *total = v;
+  return 0;
+#else
+  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+  T inc = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const T x = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= (uint32_t)o) inc += x;
+  }
+  if (lane == 31) smem[w] = inc;
+  __syncthreads();
+  T base = 0;
+  for (uint32_t k = 0; k < w; ++k) base += smem[k];
+  if (total) {
+    T t = base;
+    for (uint32_t k = w; k < (blockDim.x + 31) / 32; ++k) t += smem[k];
+    *total = t;
+  }
+  return base + inc - v;
 #endif
 }
 
 // Normative state digest (DESIGN.md "Digests"); must equal jro_state_digest.
 __global__ void state_digest_kernel(const Dev d, unsigned long long* out) {
-  __shared__ uint64_t sm[32];
+  __shared__ uint64_t sm[1][32];
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t plane = (size_t)d.R * d.Gp;
   uint64_t h = 0;
   if (i < plane && (uint32_t)(i % d.Gp) < d.G) {
     const uint32_t r = (uint32_t)(i / d.Gp), g = (uint32_t)(i % d.Gp);
     const uint4 a = d.p0[i], b = d.p1[i], c = d.p2[i];
-    const uint32_t role = c.w & 255u, fault = (c.w >> 8) & 255u, prmask = (c.w >> 16) & 255u;
-    const uint32_t nq = (c.w >> 24) & 7u, dead = (c.w >> 27) & 1u;
+    const uint32_t role = meta_role(c.w), fault = meta_fault(c.w), prmask = meta_prmask(c.w);
+    const uint32_t nq = meta_nq(c.w), dead = meta_dead(c.w);
     h = mix64(0x243f6a8885a308d3ull ^ (((d.goff + g) << 8) | (r + 1)));
     h = fold(h, (uint64_t)a.x | ((uint64_t)a.y << 32));
     h = fold(h, a.z);
@@ -327,36 +373,36 @@ __global__ void state_digest_kernel(const Dev d, unsigned long long* out) {
     uint64_t chain = 0;
     const uint32_t mk = d.mk[i], floor = d.tb[g];
     for (uint32_t bid = floor; bid <= mk && bid - floor < d.cap; ++bid) {
-      const uint32_t nx = d.cnext[(size_t)(bid & d.capm) * plane + i];
+      const uint32_t nx = d.cnext[table_row(d, plane, bid, i)];
       if (nx == ABSENT) continue;
-      const uint64_t tok = d.ctok[(size_t)(bid & d.capm) * plane + i];
+      const uint64_t tok = d.ctok[table_row(d, plane, bid, i)];
       chain += mix64(mix64((uint64_t)bid + 0x13198a2e03707344ull) ^ ((uint64_t)nx * 0xa4093822299f31d1ull) ^ tok);
     }
     h = fold(h, chain);
   }
-  block_add(out, h, sm);
+  uint64_t v[1] = {h};
+  cta_sum(v, sm);
+  if (threadIdx.x == 0) atomicAdd(out, (unsigned long long)v[0]);
 }
 
 // out[0..3] = sum msg digest, sum fsm digest, n msgs, n fsm; out[4] = faulted replicas
 __global__ void stream_digest_kernel(const Dev d, unsigned long long* out) {
-  __shared__ uint64_t sm[32];
+  __shared__ uint64_t sm[5][32];
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t plane = (size_t)d.R * d.Gp;
-  uint64_t a = 0, b = 0, x = 0, y = 0, f = 0;
+  uint64_t v[5] = {0, 0, 0, 0, 0};
   if (i < plane && (uint32_t)(i % d.Gp) < d.G) {
-    const uint4 v = d.dg[i];
+    const uint4 g = d.dg[i];
     const uint2 n = d.cn[i];
-    a = (uint64_t)v.x | ((uint64_t)v.y << 32);
-    b = (uint64_t)v.z | ((uint64_t)v.w << 32);
-    x = n.x;
-    y = n.y;
-    f = ((d.p2[i].w >> 8) & 255u) != 0;
+    v[0] = (uint64_t)g.x | ((uint64_t)g.y << 32);
+    v[1] = (uint64_t)g.z | ((uint64_t)g.w << 32);
+    v[2] = n.x;
+    v[3] = n.y;
+    v[4] = meta_fault(d.p2[i].w) != 0;
   }
-  block_add(out + 0, a, sm);
-  block_add(out + 1, b, sm);
-  block_add(out + 2, x, sm);
-  block_add(out + 3, y, sm);
-  block_add(out + 4, f, sm);
+  cta_sum(v, sm);
+  if (threadIdx.x == 0)
+    for (int c = 0; c < 5; ++c) atomicAdd(out + c, (unsigned long long)v[c]);
 }
 
 // Leader::write_state (leader.rs:101-121) for every group: the live leader with
@@ -368,8 +414,7 @@ __global__ void leader_table_kernel(const Dev d, jr_leader_entry* out, uint32_t*
   for (uint32_t r = 0; r < d.R; ++r) {
     const size_t i = (size_t)r * d.Gp + g;
     const uint4 c = d.p2[i];
-    const uint32_t role = c.w & 255u, fault = (c.w >> 8) & 255u, dead = (c.w >> 27) & 1u;
-    if (role != JR_ROLE_LEADER || fault || dead) continue;
+    if (meta_role(c.w) != JR_ROLE_LEADER || !meta_live(c.w)) continue;
     const uint4 a = d.p0[i];
     const uint64_t term = (uint64_t)a.x | ((uint64_t)a.y << 32);
     if (e.leader_id == 0 || term >= e.term) {
@@ -406,8 +451,8 @@ __global__ void kill_leaders_kernel(const Dev d, uint64_t base, uint32_t permill
     if (pick) {
       const size_t i = (size_t)r * d.Gp + g;
       const uint32_t m = d.p2[i].w;
-      hit = (m & 255u) == JR_ROLE_LEADER && ((m >> 8) & 255u) == 0 && ((m >> 27) & 1u) == 0;
-      if (hit) d.p2[i].w = m | (1u << 27);
+      hit = meta_role(m) == JR_ROLE_LEADER && meta_live(m);
+      if (hit) d.p2[i].w = m | META_DEAD;
     }
 #ifdef JR_EMU
     killed += hit ? 1u : 0u;
@@ -422,8 +467,8 @@ __global__ void kill_leaders_kernel(const Dev d, uint64_t base, uint32_t permill
 
 __global__ void set_alive_kernel(const Dev d, uint32_t g, uint32_t r, int alive) {
   const size_t i = (size_t)r * d.Gp + g;
-  uint32_t m = d.p2[i].w;
-  d.p2[i].w = alive ? (m & ~(1u << 27)) : (m | (1u << 27));
+  const uint32_t m = d.p2[i].w;
+  d.p2[i].w = alive ? (m & ~META_DEAD) : (m | META_DEAD);
 }
 
 // jr_query_many: thread k reads replica (groups[k], nodes[k] - 1)
@@ -439,7 +484,7 @@ __global__ void query_kernel(const Dev d, const uint32_t* groups, const uint32_t
   memset(&s, 0, sizeof s);
   s.current_term = (uint64_t)a.x | ((uint64_t)a.y << 32);
   s.voted_for = a.z;
-  s.role = c.w & 255u;
+  s.role = meta_role(c.w);
   s.leader_id = s.role == JR_ROLE_FOLLOWER ? a.w : 0;
   s.election_time_ms = (uint64_t)b.x | ((uint64_t)b.y << 32);
   s.election_timeout_ms = b.z;
@@ -448,12 +493,12 @@ __global__ void query_kernel(const Dev d, const uint32_t* groups, const uint32_t
   s.commit = c.y;
   s.id_gen = c.z;
   s.max_key = d.mk[i];
-  s.fault = (c.w >> 8) & 255u;
-  s.alive = ((c.w >> 27) & 1u) ? 0 : 1;
-  s.n_queued = (c.w >> 24) & 7u;
+  s.fault = meta_fault(c.w);
+  s.alive = meta_dead(c.w) ? 0 : 1;
+  s.n_queued = meta_nq(c.w);
   if (s.role == JR_ROLE_LEADER) {
     s.heartbeat_time_ms = (uint64_t)e.x | ((uint64_t)e.y << 32);
-    s.progress_replicate = (c.w >> 16) & 255u;
+    s.progress_replicate = meta_prmask(c.w);
     for (uint32_t k = 0; k < d.R; ++k) {
       const uint4 v = d.pr[(size_t)(k / 4) * plane + i];
       s.progress_head[k] = (k & 3) == 0 ? v.x : (k & 3) == 1 ? v.y : (k & 3) == 2 ? v.z : v.w;
@@ -478,10 +523,10 @@ __global__ void chain_read_kernel(const Dev d, const uint4* reqs, const uint32_t
   for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) {
     const uint64_t bid = (uint64_t)rq.z + k;
     uint32_t nx = ABSENT;
-    if (bid >= floor && bid - floor < d.cap) nx = d.cnext[(size_t)((uint32_t)bid & d.capm) * plane + i];
+    if (bid >= floor && bid - floor < d.cap) nx = d.cnext[table_row(d, plane, (uint32_t)bid, i)];
     present[rq.w + k] = nx != ABSENT;
     out[rq.w + k] = jr_block{bid, nx != ABSENT ? nx : 0ull,
-                             nx != ABSENT ? d.ctok[(size_t)((uint32_t)bid & d.capm) * plane + i] : 0ull};
+                             nx != ABSENT ? d.ctok[table_row(d, plane, (uint32_t)bid, i)] : 0ull};
   }
 }
 
@@ -497,14 +542,14 @@ __global__ void truncate_kernel(const Dev d, uint32_t margin, const uint8_t* ski
   uint32_t lo = 0xFFFFFFFFu;
   for (uint32_t r = 0; r < d.R; ++r) {
     const uint4 c = d.p2[(size_t)r * d.Gp + g];
-    if (((c.w >> 8) & 255u) != 0 || ((c.w >> 27) & 1u)) continue;  // faulted or silenced: not waited for
+    if (!meta_live(c.w)) continue;  // faulted or silenced: not waited for
     lo = min(lo, c.y);
   }
   if (lo == 0xFFFFFFFFu) return;
   const uint32_t floor = lo > margin ? lo - margin : 0u;
   if (floor <= old) return;
   for (uint32_t b = old; b < floor && b - old < d.cap; ++b)
-    for (uint32_t r = 0; r < d.R; ++r) d.cnext[(size_t)(b & d.capm) * plane + (size_t)r * d.Gp + g] = ABSENT;
+    for (uint32_t r = 0; r < d.R; ++r) d.cnext[table_row(d, plane, b, (size_t)r * d.Gp + g)] = ABSENT;
   // a replica that was not waited for (silenced / faulted) may have lost every block it held: an empty table's largest key is 0
   for (uint32_t r = 0; r < d.R; ++r)
     if (d.mk[(size_t)r * d.Gp + g] < floor) d.mk[(size_t)r * d.Gp + g] = 0;
@@ -532,7 +577,7 @@ __global__ void export_count_kernel(const Dev d, const uint2* targets, uint32_t 
   const size_t i = (size_t)t.y * d.Gp + t.x;
   const uint32_t floor = d.tb[t.x], span = window_span(d, i, floor);
   uint32_t cnt = 0;
-  for (uint32_t b = 0; b < span; ++b) cnt += d.cnext[(size_t)((floor + b) & d.capm) * plane + i] != ABSENT ? 1u : 0u;
+  for (uint32_t b = 0; b < span; ++b) cnt += d.cnext[table_row(d, plane, floor + b, i)] != ABSENT ? 1u : 0u;
   const uint4 c = d.p2[i];
   jr_persisted_chain o;
   o.group = t.x;
@@ -540,7 +585,7 @@ __global__ void export_count_kernel(const Dev d, const uint2* targets, uint32_t 
   o.commit = c.y;
   o.first_block = 0;
   o.n_blocks = cnt;
-  o.commit_key = (c.w >> 28) & 1u;
+  o.commit_key = meta_ckey(c.w);
   out[k] = o;
 }
 
@@ -554,7 +599,7 @@ __global__ void export_pack_kernel(const Dev d, const jr_persisted_chain* desc, 
   const uint32_t floor = d.tb[c.group], span = window_span(d, i, floor);
   jr_block* o = out + c.first_block;
   for (uint32_t b = 0, j = 0; b < span && j < c.n_blocks; ++b) {
-    const size_t row = (size_t)((floor + b) & d.capm) * plane + i;
+    const size_t row = table_row(d, plane, floor + b, i);
     const uint32_t nx = d.cnext[row];
     if (nx != ABSENT) o[j++] = jr_block{(uint64_t)floor + b, nx, d.ctok[row]};
   }
@@ -579,18 +624,18 @@ __global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persiste
   if (q.n_blocks == JR_RESTART_IN_PLACE) {
     const uint4 c = d.p2[i];
     commit = c.y;
-    ckey = (c.w >> 28) & 1u;
+    ckey = meta_ckey(c.w);
     for (uint32_t b = window_span(d, i, floor); b-- > 0;)   // the largest key becomes exact, as an export would make it
-      if (d.cnext[(size_t)((floor + b) & d.capm) * plane + i] != ABSENT) { mk = floor + b; break; }
+      if (d.cnext[table_row(d, plane, floor + b, i)] != ABSENT) { mk = floor + b; break; }
   } else {
     commit = (uint32_t)q.commit;
     ckey = q.commit_key ? 1u : 0u;
-    for (uint32_t b = 0; b < d.cap; ++b) d.cnext[(size_t)((floor + b) & d.capm) * plane + i] = ABSENT;
+    for (uint32_t b = 0; b < d.cap; ++b) d.cnext[table_row(d, plane, floor + b, i)] = ABSENT;
     const jr_block* bl = blocks + q.first_block;
     for (uint32_t j = 0; j < q.n_blocks; ++j) {
       const uint32_t bid = (uint32_t)bl[j].id;
-      d.cnext[(size_t)(bid & d.capm) * plane + i] = (uint32_t)bl[j].next;
-      d.ctok[(size_t)(bid & d.capm) * plane + i] = bl[j].data;
+      d.cnext[table_row(d, plane, bid, i)] = (uint32_t)bl[j].next;
+      d.ctok[table_row(d, plane, bid, i)] = bl[j].data;
       mk = bid;                        // ascending: the last one is the largest
     }
   }
@@ -602,7 +647,7 @@ __global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persiste
   const uint32_t timeout = election_timeout_draw(d.seed, d.goff + g, r + 1, 0, d.emin, d.emax);
   d.p0[i] = make_uint4(0, 0, 0, 0);
   d.p1[i] = make_uint4((uint32_t)now, (uint32_t)(now >> 32), timeout, 1);
-  d.p2[i] = make_uint4(commit, commit, idgen, JR_ROLE_FOLLOWER | ((ckey ? 1u : 0u) << 28));
+  d.p2[i] = make_uint4(commit, commit, idgen, meta_pack(JR_ROLE_FOLLOWER, 0, 0, 0, 0, ckey));
   d.p3[i] = make_uint4(0, 0, 0, 0);
   d.mk[i] = mk;
   d.oc[0][i] = 0;
@@ -643,16 +688,16 @@ __global__ void verify_walk_kernel(const Dev d, const uint32_t* groups, uint32_t
   const size_t plane = (size_t)d.R * d.Gp, i = (size_t)r * d.Gp + g;
   const uint32_t meta = d.p2[i].w, cm = d.p2[i].y, floor = d.tb[g];
   uint2 v = make_uint2(VW_SKIP, 0u);
-  if (((meta >> 8) & 255u) == 0 && ((meta >> 27) & 1u) == 0) {
+  if (meta_live(meta)) {
     if (cm < floor) {
       v = make_uint2(JR_VERIFY_BELOW_FLOOR, cm);
-    } else if (cm - floor >= d.cap || d.cnext[(size_t)(cm & d.capm) * plane + i] == ABSENT) {
+    } else if (cm - floor >= d.cap || d.cnext[table_row(d, plane, cm, i)] == ABSENT) {
       v = make_uint2(JR_VERIFY_COMMIT_ABSENT, cm);
     } else {
       v = make_uint2(VW_INTACT, cm);
       uint32_t x = cm;
       for (uint32_t s = 0; s < d.cap; ++s) {   // ids fall strictly inside [floor, floor + cap): at most cap steps
-        const uint32_t nx = d.cnext[(size_t)(x & d.capm) * plane + i];
+        const uint32_t nx = d.cnext[table_row(d, plane, x, i)];
         // absent (ABSENT is above every id) or a next that is not below its id, genesis 0 -> 0 excepted
         if (nx >= x && (x | nx) != 0) { v = make_uint2(JR_VERIFY_CHAIN_BROKEN, x); break; }
         if (x == 0 || nx < floor) break;
@@ -667,7 +712,7 @@ __global__ void verify_walk_kernel(const Dev d, const uint32_t* groups, uint32_t
 // lowest leader of a term two or more checked leaders share.  rep += this CTA's counts (one atomic per count and CTA).
 __global__ void verify_judge_kernel(const Dev d, const uint32_t* groups, uint32_t n, const uint2* vw, uint2* vf,
                                     unsigned long long* rep) {
-  __shared__ unsigned long long s[VERIFY_COUNTS][32];
+  __shared__ uint64_t s[VERIFY_COUNTS][32];
   const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   uint64_t cnt[VERIFY_COUNTS] = {0, 0, 0, 0, 0, 0, 0};   // checked, skipped, below floor, absent, broken, diverged, conflicts
   if (t < (size_t)d.R * n) {
@@ -684,25 +729,25 @@ __global__ void verify_judge_kernel(const Dev d, const uint32_t* groups, uint32_
       const size_t ir = (size_t)(ref - 1) * d.Gp + g;
       const uint32_t cm = mine.y, floor = d.tb[g];
       uint32_t y = refc;   // down the reference's chain to the first id <= c_n: c_n is on it iff that id is c_n
-      for (uint32_t s2 = 0; s2 < d.cap && y > cm; ++s2) y = d.cnext[(size_t)(y & d.capm) * plane + ir];
+      for (uint32_t s2 = 0; s2 < d.cap && y > cm; ++s2) y = d.cnext[table_row(d, plane, y, ir)];
       if (y != cm) {
         kind = JR_VERIFY_DIVERGED;
       } else {             // then both chains share every block down to the first row that differs
         uint32_t x = cm;
         for (uint32_t s2 = 0; s2 < d.cap; ++s2) {
-          const size_t row = (size_t)(x & d.capm) * plane;
-          const uint32_t nx = d.cnext[row + i];
-          if (nx != d.cnext[row + ir] || d.ctok[row + i] != d.ctok[row + ir]) { kind = JR_VERIFY_DIVERGED; id = x; break; }
+          const size_t ri = table_row(d, plane, x, i), rr = table_row(d, plane, x, ir);
+          const uint32_t nx = d.cnext[ri];
+          if (nx != d.cnext[rr] || d.ctok[ri] != d.ctok[rr]) { kind = JR_VERIFY_DIVERGED; id = x; break; }
           if (x == 0 || nx < floor) break;
           x = nx;
         }
       }
     }
-    if (mine.x != VW_SKIP && (d.p2[i].w & 255u) == JR_ROLE_LEADER) {
+    if (mine.x != VW_SKIP && meta_role(d.p2[i].w) == JR_ROLE_LEADER) {
       const uint32_t term_lo = d.p0[i].x, term_hi = d.p0[i].y;
       for (uint32_t k = 0; k < d.R; ++k) {
         const size_t ik = (size_t)k * d.Gp + g;
-        if (vw[(size_t)k * n + j].x != VW_SKIP && (d.p2[ik].w & 255u) == JR_ROLE_LEADER && d.p0[ik].x == term_lo &&
+        if (vw[(size_t)k * n + j].x != VW_SKIP && meta_role(d.p2[ik].w) == JR_ROLE_LEADER && d.p0[ik].x == term_lo &&
             d.p0[ik].y == term_hi)
           lc |= 1u << k;
       }
@@ -715,24 +760,10 @@ __global__ void verify_judge_kernel(const Dev d, const uint32_t* groups, uint32_
     for (int c = 2; c < 6; ++c) cnt[c] = kind == (uint32_t)(c - 1);   // (static indices: the counts stay in registers)
     cnt[6] = lc != 0;
   }
-#ifdef JR_EMU
-  (void)s;
-  for (int c = 0; c < VERIFY_COUNTS; ++c)
-    if (cnt[c]) atomicAdd(rep + c, (unsigned long long)cnt[c]);
-#else
-#pragma unroll
-  for (int c = 0; c < VERIFY_COUNTS; ++c) {
-    uint64_t v = cnt[c];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) s[c][threadIdx.x >> 5] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < VERIFY_COUNTS) {
-    unsigned long long v = 0;
-    for (uint32_t w = 0; w < (blockDim.x + 31) / 32; ++w) v += s[threadIdx.x][w];
-    if (v) atomicAdd(rep + threadIdx.x, v);
-  }
-#endif
+  cta_sum(cnt, s);
+  if (threadIdx.x == 0)
+    for (int c = 0; c < VERIFY_COUNTS; ++c)
+      if (cnt[c]) atomicAdd(rep + c, (unsigned long long)cnt[c]);
 }
 
 __device__ __forceinline__ uint32_t verify_findings_of(const Dev& d, const uint2* vf, uint32_t n, uint32_t j) {
@@ -746,20 +777,11 @@ __device__ __forceinline__ uint32_t verify_findings_of(const Dev& d, const uint2
 
 // One thread per listed group: part[CTA] = the CTA's findings.
 __global__ void verify_count_kernel(const Dev d, uint32_t n, const uint2* vf, unsigned long long* part) {
-  __shared__ uint32_t s_warp[32];
+  __shared__ uint32_t s[1][32];
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t c = j < n ? verify_findings_of(d, vf, n, j) : 0u;
-#ifdef JR_EMU
-  (void)s_warp;
-#else
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x != 0) return;
-  c = 0;
-  for (uint32_t w = 0; w < (blockDim.x + 31) / 32; ++w) c += s_warp[w];
-#endif
-  part[blockIdx.x] = c;
+  uint32_t c[1] = {j < n ? verify_findings_of(d, vf, n, j) : 0u};
+  cta_sum(c, s);
+  if (threadIdx.x == 0) part[blockIdx.x] = c[0];
 }
 
 // One thread: exclusive scan of the per-CTA counts (it only runs when some group has findings).
@@ -775,22 +797,7 @@ __global__ void verify_pack_kernel(const Dev d, const uint32_t* groups, uint32_t
   __shared__ uint32_t s_warp[32];
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t c = j < n ? verify_findings_of(d, vf, n, j) : 0u;
-  uint32_t pre = 0;
-#ifdef JR_EMU
-  (void)s_warp;
-#else
-  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-  uint32_t inc = c;
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= (uint32_t)o) inc += v;
-  }
-  if (lane == 31) s_warp[w] = inc;
-  __syncthreads();
-  uint32_t base = 0;
-  for (uint32_t k = 0; k < w; ++k) base += s_warp[k];
-  pre = base + inc - c;
-#endif
+  const uint32_t pre = cta_exclusive_scan(c, s_warp);
   if (j >= n || c == 0) return;
   const uint32_t g = verify_group(groups, j);
   jr_verify_finding* o = out + part[blockIdx.x] + pre;
@@ -818,14 +825,13 @@ __global__ void verify_pack_kernel(const Dev d, const uint32_t* groups, uint32_t
 // array in thread order i = replica * Gp + group -- sorted by (node, group), FIFO per replica -- with an exclusive
 // scan over the per-replica counts, writes them to a device staging buffer and empties the FIFOs; the copy engine
 // takes the batch to pinned host memory (fsm_records_enqueue).
-constexpr uint32_t SCAN_THREADS = 1024;
 struct FsmHeader {          // written by fsm_pack_kernel next to the records
   unsigned long long n_records, n_dropped, n_instructions;
   uint32_t node_offset[JR_MAX_REPLICAS + 1];
   unsigned long long n_wanted;   // records the FIFOs held, before the cut at the batch's capacity
 };
 
-// Three small kernels (CTAs of T threads; the CPU emulation runs them with T = 1):
+// Three small kernels on cta_sum / cta_exclusive_scan:
 //   fsm_count_kernel  per-CTA sums of the replicas' record counts            -> part[3][n_ctas]
 //   fsm_scan_kernel   one CTA: exclusive scan of those sums, batch totals     -> part[0] becomes CTA offsets, hdr
 //   fsm_pack_kernel   CTA-local scan + CTA offset = each replica's position; copies its records, empties its FIFO
@@ -837,123 +843,54 @@ __device__ __forceinline__ uint32_t fsm_kept(const Dev& d, size_t i, uint2 c) {
 
 // `xdrop` (may be null): elements each replica lost besides the runs beyond F.
 __global__ void fsm_count_kernel(const Dev d, const uint2* cnt, const uint32_t* xdrop, unsigned long long* part, uint32_t n_ctas) {
-  __shared__ unsigned long long s[3][SCAN_THREADS / 32];
+  __shared__ unsigned long long s[3][32];
   const size_t plane = (size_t)d.R * d.Gp;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  unsigned long long rec = 0, drop = 0, ins = 0;
+  unsigned long long v[3] = {0, 0, 0};   // records, dropped, Instructions
   if (i < plane && (uint32_t)(i % d.Gp) < d.G) {
     const uint2 c = cnt[i];
-    rec = min(c.x, d.F);
-    drop = (c.x > d.F ? c.x - d.F : 0u) + (xdrop ? xdrop[i] : 0u);
-    ins = c.y;
+    v[0] = min(c.x, d.F);
+    v[1] = (c.x > d.F ? c.x - d.F : 0u) + (xdrop ? xdrop[i] : 0u);
+    v[2] = c.y;
   }
-#ifdef JR_EMU
-  (void)s;
-#else
-  for (int o = 16; o > 0; o >>= 1) {
-    rec += __shfl_down_sync(0xffffffffu, rec, o);
-    drop += __shfl_down_sync(0xffffffffu, drop, o);
-    ins += __shfl_down_sync(0xffffffffu, ins, o);
-  }
-  if ((threadIdx.x & 31) == 0) { s[0][threadIdx.x >> 5] = rec; s[1][threadIdx.x >> 5] = drop; s[2][threadIdx.x >> 5] = ins; }
-  __syncthreads();
+  cta_sum(v, s);
   if (threadIdx.x != 0) return;
-  rec = drop = ins = 0;
-  for (uint32_t w = 0; w < (blockDim.x + 31) / 32; ++w) { rec += s[0][w]; drop += s[1][w]; ins += s[2][w]; }
-#endif
-  part[blockIdx.x] = rec;
-  part[n_ctas + blockIdx.x] = drop;
-  part[2 * (size_t)n_ctas + blockIdx.x] = ins;
+  part[blockIdx.x] = v[0];
+  part[n_ctas + blockIdx.x] = v[1];
+  part[2 * (size_t)n_ctas + blockIdx.x] = v[2];
 }
 
 // elem_drops: records cut off by cap_records are counted by their elements, in fsm_pack_kernel (the client responses: their
 // n_dropped counts responses), instead of one each here.
 __global__ void fsm_scan_kernel(unsigned long long* part, uint32_t n_ctas, FsmHeader* hdr, uint32_t cap_records, bool elem_drops) {
-  __shared__ unsigned long long s_sum[SCAN_THREADS];
+  __shared__ unsigned long long s_warp[32];
   const uint32_t t = threadIdx.x, T = blockDim.x;
   const uint32_t per = (n_ctas + T - 1) / T;
   const uint32_t lo = min(n_ctas, per * t), hi = min(n_ctas, per * (t + 1));
   unsigned long long sum = 0, drop = 0, ins = 0;
   for (uint32_t k = lo; k < hi; ++k) { sum += part[k]; drop += part[n_ctas + k]; ins += part[2 * (size_t)n_ctas + k]; }
-#ifdef JR_EMU
-  s_sum[t] = sum;
-  __syncthreads();
+  unsigned long long total;
+  unsigned long long at = cta_exclusive_scan(sum, s_warp, &total);
   if (t == 0) {
-    unsigned long long run = 0;
-    for (uint32_t k = 0; k < T; ++k) { const unsigned long long v = s_sum[k]; s_sum[k] = run; run += v; }
-    hdr->n_records = min(run, (unsigned long long)cap_records);
-    hdr->n_dropped = run > cap_records && !elem_drops ? run - cap_records : 0ull;   // + the per-replica drops, added below
-    hdr->n_wanted = run;
+    hdr->n_records = min(total, (unsigned long long)cap_records);
+    hdr->n_dropped = total > cap_records && !elem_drops ? total - cap_records : 0ull;   // + the per-replica drops, added below
+    hdr->n_wanted = total;
     hdr->n_instructions = 0;
   }
   __syncthreads();
-#else
-  {  // exclusive scan of the T per-thread sums: warp shuffles, then the warp totals (T <= 1024: one warp's worth)
-    __shared__ unsigned long long s_warp[32];
-    const uint32_t lane = t & 31u, w = t >> 5;
-    unsigned long long inc = sum;
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long v = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= (uint32_t)o) inc += v;
-    }
-    if (lane == 31) s_warp[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-      const unsigned long long mine = lane < (T + 31) / 32 ? s_warp[lane] : 0ull;
-      unsigned long long wi = mine;
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long v = __shfl_up_sync(0xffffffffu, wi, o);
-        if (lane >= (uint32_t)o) wi += v;
-      }
-      s_warp[lane] = wi - mine;                           // exclusive prefix of the warp totals
-      if (lane == 31) {
-        hdr->n_records = min(wi, (unsigned long long)cap_records);
-        hdr->n_dropped = wi > cap_records && !elem_drops ? wi - cap_records : 0ull;   // + the per-replica drops, added below
-        hdr->n_wanted = wi;
-        hdr->n_instructions = 0;
-      }
-    }
-    __syncthreads();
-    s_sum[t] = s_warp[w] + inc - sum;
-  }
-  __syncthreads();
-#endif
-#ifdef JR_EMU
-  hdr->n_dropped += drop;
-  hdr->n_instructions += ins;
-#else
   if (drop) atomicAdd(&hdr->n_dropped, drop);
   if (ins) atomicAdd(&hdr->n_instructions, ins);
-#endif
-  unsigned long long at = s_sum[t];
   for (uint32_t k = lo; k < hi; ++k) { const unsigned long long v = part[k]; part[k] = at; at += v; }
 }
 
 // Thread i moves its replica's records to out[position ..] and empties the FIFO.  `out` may be mapped host memory.
 __global__ void fsm_pack_kernel(const Dev d, const uint4* fifo, uint2* cnt, const unsigned long long* part, FsmHeader* hdr,
                                 uint4* out, uint32_t cap_records, bool elem_drops) {
-  __shared__ uint32_t s_warp[SCAN_THREADS / 32];
+  __shared__ uint32_t s_warp[32];
   const size_t plane = (size_t)d.R * d.Gp;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t n = i < plane ? fsm_kept(d, i, cnt[i]) : 0u;
-  // exclusive scan of n over the CTA
-  uint32_t pre = 0;
-#ifdef JR_EMU
-  (void)s_warp;
-#else
-  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-  uint32_t inc = n;
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= (uint32_t)o) inc += v;
-  }
-  if (lane == 31) s_warp[w] = inc;
-  __syncthreads();
-  uint32_t base = 0;
-  for (uint32_t k = 0; k < w; ++k) base += s_warp[k];
-  pre = base + inc - n;
-#endif
-  const unsigned long long at64 = part[blockIdx.x] + pre;
+  const unsigned long long at64 = part[blockIdx.x] + cta_exclusive_scan(n, s_warp);
   if (i < plane) {
     const uint32_t at = (uint32_t)min(at64, (unsigned long long)cap_records);
     for (uint32_t k = 0; k < n && at + k < cap_records; ++k) {
@@ -1186,14 +1123,12 @@ __global__ void fsm_respond_kernel(const Dev d, const RespPlanes q, const FsmHea
 }
 
 __global__ void max_u32_kernel(const uint32_t* v, size_t n, uint32_t* out) {
-  uint32_t m = 0;
+  __shared__ uint32_t s[1][32];
+  uint32_t m[1] = {0};
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    m = max(m, v[i]);
-#ifndef JR_EMU
-  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_down_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0)
-#endif
-    atomicMax(out, m);
+    m[0] = max(m[0], v[i]);
+  cta_sum(m, s, MaxOp());
+  if (threadIdx.x == 0) atomicMax(out, m[0]);
 }
 
 // ============================================================================
@@ -1812,7 +1747,7 @@ static void decode_unit(const uint4& h, uint32_t group, uint32_t sender, const u
 static jr_status device_max(jr_engine* e, const uint32_t* v, size_t n, uint32_t* out) {
   uint32_t* s = reinterpret_cast<uint32_t*>(e->scratch);
   CK(cudaMemsetAsync(s, 0, sizeof(uint32_t), e->stream));
-  JR_LAUNCH(max_u32_kernel, 64, 256, e->stream, v, n, s);
+  JR_LAUNCH(max_u32_kernel, 64, CTA_THREADS, e->stream, v, n, s);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, s, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -1862,11 +1797,7 @@ static jr_status fsm_records_enqueue(jr_engine* e) {
   e->fsm_i = (b + 1) % jr_engine::NSLOT;
   const size_t plane = (size_t)d.R * d.Gp;
   if (e->fsm_used[b]) CK(cudaStreamWaitEvent(e->stream, e->fsm_landed[b], 0));  // stage[b] has left the device
-#ifdef JR_EMU
-  const uint32_t T = 1, Ts = 1;
-#else
-  const uint32_t T = 256, Ts = SCAN_THREADS;
-#endif
+  const uint32_t T = CTA_THREADS, Ts = SCAN_THREADS;
   const uint32_t n_ctas = (uint32_t)((plane + T - 1) / T);
   JR_LAUNCH(fsm_count_kernel, n_ctas, T, e->stream, d, d.fc, nullptr, e->fsm_part, n_ctas);
   CK(cudaGetLastError());
@@ -2681,7 +2612,7 @@ jr_status jr_state_digest(jr_engine* e, uint64_t* out) {
   CK(cudaSetDevice(e->cfg.device));
   const size_t plane = (size_t)e->d.R * e->d.Gp;
   CK(cudaMemsetAsync(e->scratch, 0, 8 * sizeof(unsigned long long), e->stream));
-  JR_LAUNCH(state_digest_kernel, (unsigned)((plane + 255) / 256), 256, e->stream, e->d, e->scratch);
+  JR_LAUNCH(state_digest_kernel, (unsigned)((plane + CTA_THREADS - 1) / CTA_THREADS), CTA_THREADS, e->stream, e->d, e->scratch);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, e->scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -2692,7 +2623,7 @@ static jr_status stream_sums(jr_engine* e, uint64_t v[5]) {
   CK(cudaSetDevice(e->cfg.device));
   const size_t plane = (size_t)e->d.R * e->d.Gp;
   CK(cudaMemsetAsync(e->scratch, 0, 8 * sizeof(unsigned long long), e->stream));
-  JR_LAUNCH(stream_digest_kernel, (unsigned)((plane + 255) / 256), 256, e->stream, e->d, e->scratch);
+  JR_LAUNCH(stream_digest_kernel, (unsigned)((plane + CTA_THREADS - 1) / CTA_THREADS), CTA_THREADS, e->stream, e->d, e->scratch);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(v, e->scratch, 5 * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -2932,11 +2863,7 @@ jr_status jr_verify_groups(jr_engine* e, const uint32_t* groups, size_t n_groups
   *n_findings = 0;
   if (n == 0) return JR_OK;
   CK(cudaSetDevice(e->cfg.device));
-#ifdef JR_EMU
-  const uint32_t T = 1;   // the CTA-wide scans of count and pack
-#else
-  const uint32_t T = 256;
-#endif
+  const uint32_t T = CTA_THREADS;
   const size_t reps = (size_t)d.R * n;
   const uint32_t n_ctas = (uint32_t)((n + T - 1) / T);
   const size_t o_part = 16 * sizeof(unsigned long long), o_list = o_part + ((size_t)n_ctas * 8 + 15) / 16 * 16;
@@ -2951,10 +2878,10 @@ jr_status jr_verify_groups(jr_engine* e, const uint32_t* groups, size_t n_groups
   uint2* vf = (uint2*)(base + o_vf);
   CK(cudaMemsetAsync(rep, 0, VERIFY_COUNTS * sizeof(unsigned long long), e->stream));
   if (groups) CK(cudaMemcpyAsync(base + o_list, list.data(), n * 4, cudaMemcpyHostToDevice, e->stream));
-  const unsigned grid = (unsigned)((reps + 255) / 256);
-  JR_LAUNCH(verify_walk_kernel, grid, 256, e->stream, d, dlist, (uint32_t)n, vw);
+  const unsigned grid = (unsigned)((reps + T - 1) / T);
+  JR_LAUNCH(verify_walk_kernel, grid, T, e->stream, d, dlist, (uint32_t)n, vw);
   CK(cudaGetLastError());
-  JR_LAUNCH(verify_judge_kernel, grid, 256, e->stream, d, dlist, (uint32_t)n, (const uint2*)vw, vf, rep);
+  JR_LAUNCH(verify_judge_kernel, grid, T, e->stream, d, dlist, (uint32_t)n, (const uint2*)vw, vf, rep);
   CK(cudaGetLastError());
   unsigned long long cnt[VERIFY_COUNTS];
   CK(cudaMemcpyAsync(cnt, rep, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));

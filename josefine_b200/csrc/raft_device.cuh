@@ -72,6 +72,26 @@ struct Dev {
   uint64_t seed, goff;
 };
 
+// A replica's meta word, P2.w: role (bits 0-7), fault (8-15), pre-vote mask (16-23), queued client requests (24-26),
+// dead (27), commit key (28).
+constexpr uint32_t META_DEAD = 1u << 27;
+__device__ __forceinline__ uint32_t meta_role(uint32_t m) { return m & 255u; }
+__device__ __forceinline__ uint32_t meta_fault(uint32_t m) { return (m >> 8) & 255u; }
+__device__ __forceinline__ uint32_t meta_prmask(uint32_t m) { return (m >> 16) & 255u; }
+__device__ __forceinline__ uint32_t meta_nq(uint32_t m) { return (m >> 24) & 7u; }
+__device__ __forceinline__ uint32_t meta_dead(uint32_t m) { return (m >> 27) & 1u; }
+__device__ __forceinline__ uint32_t meta_ckey(uint32_t m) { return (m >> 28) & 1u; }
+__device__ __forceinline__ bool meta_live(uint32_t m) { return meta_fault(m) == 0 && !meta_dead(m); }
+__device__ __forceinline__ uint32_t meta_pack(uint32_t role, uint32_t fault, uint32_t prmask, uint32_t nq, uint32_t dead,
+                                              uint32_t ckey) {
+  return role | (fault << 8) | (prmask << 16) | (nq << 24) | (dead << 27) | (ckey << 28);
+}
+
+// Index in d.cnext / d.ctok of block `id` of the replica at plane index i (plane = R * Gp).
+__device__ __forceinline__ size_t table_row(const Dev& d, size_t plane, uint32_t id, size_t i) {
+  return (size_t)(id & d.capm) * plane + i;
+}
+
 // Per-lane view of the CTA's shared memory.  Us == 0 / W == 0 (sparse inject
 // kernel) means "no staging": every access goes to global memory.
 struct Local {
@@ -398,9 +418,9 @@ struct Replica {
     term = (uint64_t)a.x | ((uint64_t)a.y << 32); voted = a.z;
     etime = (uint64_t)b.x | ((uint64_t)b.y << 32); etimeout = b.z; draws = b.w;
     head = c.x; commit = c.y; idgen = c.z;
-    uint32_t m = c.w;
-    role = m & 255u; fault = (m >> 8) & 255u; prmask = (m >> 16) & 255u;
-    nq = (m >> 24) & 7u; dead = (m >> 27) & 1u; ckey = (m >> 28) & 1u;
+    const uint32_t m = c.w;
+    role = meta_role(m); fault = meta_fault(m); prmask = meta_prmask(m);
+    nq = meta_nq(m); dead = meta_dead(m); ckey = meta_ckey(m);
     maxkey = d.mk[rg];
     tbase = d.tb[g];
     hbtime = 0;
@@ -430,8 +450,7 @@ struct Replica {
   __device__ __forceinline__ void store(bool last_part = true) {
     d.p0[rg] = make_uint4((uint32_t)term, (uint32_t)(term >> 32), voted, role == JR_ROLE_FOLLOWER ? leader : 0u);
     d.p1[rg] = make_uint4((uint32_t)etime, (uint32_t)(etime >> 32), etimeout, draws);
-    uint32_t m = role | (fault << 8) | (prmask << 16) | (nq << 24) | (dead << 27) | (ckey << 28);
-    d.p2[rg] = make_uint4(head, commit, idgen, m);
+    d.p2[rg] = make_uint4(head, commit, idgen, meta_pack(role, fault, prmask, nq, dead, ckey));
     d.mk[rg] = maxkey;
     if (role != JR_ROLE_FOLLOWER) {
       d.p3[rg] = make_uint4((uint32_t)hbtime, (uint32_t)(hbtime >> 32), role == JR_ROLE_CANDIDATE ? seen : 0u,
@@ -460,7 +479,7 @@ struct Replica {
   // ------------------------------------------------------------------ block table (chain.rs)
   // The table holds the ids of a window [tbase, tbase + cap): row = id & capm.  Ids below the floor were
   // truncated (jr_truncate, deviation D7) and read as absent; ids at or past the end cannot be stored.
-  __device__ __forceinline__ size_t tix(uint32_t bid) const { return (size_t)(bid & d.capm) * plane + rg; }
+  __device__ __forceinline__ size_t tix(uint32_t bid) const { return table_row(d, plane, bid, rg); }
   __device__ __forceinline__ bool in_window(uint32_t bid) const { return bid - tbase < d.cap && bid < FS_NOTIFY_BIT; }   // (ids < 2^31, D4)
   // Block table reads go through a direct-mapped, write-through cache in shared
   // memory (tag = id).  Only this lane writes its own table, so the cache is

@@ -179,7 +179,7 @@ struct SymGroup {
 #endif
   }
   __device__ __forceinline__ size_t rg(uint32_t r) const { return (size_t)r * d.Gp + g; }
-  __device__ __forceinline__ size_t row(uint32_t r, uint32_t bid) const { return (size_t)(bid & d.capm) * plane + rg(r); }
+  __device__ __forceinline__ size_t row(uint32_t r, uint32_t bid) const { return table_row(d, plane, bid, rg(r)); }
   __device__ __forceinline__ bool in_window(uint32_t bid) const { return bid - tbase < d.cap; }   // (sym_enter made sure ids stay below 2^31)
   __device__ __forceinline__ uint4& slot(uint32_t r, uint32_t bid) const { return rows[((r == L ? 0u : SYM_ROWS) + (bid % SYM_ROWS)) * STRIDE]; }
   __device__ __forceinline__ void cache_put(uint32_t r, uint32_t bid, uint32_t nx, uint64_t tk) const {
@@ -568,10 +568,10 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, true>& s, SymMail& m, cons
   for (int r = 0; r < R; ++r) {
     p2[r] = d.p2[s.rg(r)];
     const uint32_t meta = p2[r].w;
-    if (((meta >> 8) & 255u) || ((meta >> 27) & 1u)) return false;          // faulted or silenced
-    if ((meta & 255u) == JR_ROLE_LEADER) { L = r; ++nlead; }
-    else if ((meta & 255u) != JR_ROLE_FOLLOWER) return false;
-    if ((meta >> 24) & 7u) return false;                                      // queued client requests
+    if (!meta_live(meta)) return false;                                       // faulted or silenced
+    if (meta_role(meta) == JR_ROLE_LEADER) { L = r; ++nlead; }
+    else if (meta_role(meta) != JR_ROLE_FOLLOWER) return false;
+    if (meta_nq(meta)) return false;                                          // queued client requests
   }
   if (nlead != 1) return false;
   s.L = L;
@@ -587,14 +587,14 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, true>& s, SymMail& m, cons
     if ((uint32_t)r == f0i) pf = p2[r];
   }
   s.head = pl.x; s.commit = pl.y; s.idgen = pl.z;
-  s.ckey = (pl.w >> 28) & 1u;
+  s.ckey = meta_ckey(pl.w);
   s.maxkey = d.mk[s.rg(L)];
   if (!(s.idgen > s.head)) return false;                                      // the next append would assert (chain.rs:163)
   const uint4 l3 = d.p3[s.rg(L)];
   s.hbtime = (uint64_t)l3.x | ((uint64_t)l3.y << 32);
   // followers: identical
   const uint32_t f0 = s.F0;
-  s.fhead = pf.x; s.fcommit = pf.y; s.fckey = (pf.w >> 28) & 1u;
+  s.fhead = pf.x; s.fcommit = pf.y; s.fckey = meta_ckey(pf.w);
   s.fmaxkey = d.mk[s.rg(f0)];
   const uint64_t hbgap = ((uint64_t)d.hb / p.dt + 1) * p.dt;                 // ticks between two heartbeats, in ms
 #pragma unroll
@@ -602,7 +602,7 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, true>& s, SymMail& m, cons
     if ((uint32_t)r == L) continue;
     const uint4 a = d.p0[s.rg(r)];
     if (((uint64_t)a.x | ((uint64_t)a.y << 32)) != s.term || a.z != L + 1 || a.w != L + 1) return false;
-    if (p2[r].x != s.fhead || p2[r].y != s.fcommit || ((p2[r].w >> 28) & 1u) != s.fckey) return false;
+    if (p2[r].x != s.fhead || p2[r].y != s.fcommit || meta_ckey(p2[r].w) != s.fckey) return false;
     if (d.mk[s.rg(r)] != s.fmaxkey) return false;
   }
   if ((uint64_t)d.emin <= hbgap || s.hbtime > p.now) return false;   // between two heartbeats no timer (>= emin) can fire
@@ -616,7 +616,7 @@ __device__ __forceinline__ bool sym_enter(SymGroup<R, true>& s, SymMail& m, cons
     if (q * 4 + 2 < R) ph[q * 4 + 2] = v.z;
     if (q * 4 + 3 < R) ph[q * 4 + 3] = v.w;
   }
-  const uint32_t prmask = (pl.w >> 16) & 255u;
+  const uint32_t prmask = meta_prmask(pl.w);
   s.ph_self = 0; s.ph_f = 0;
 #pragma unroll
   for (int r = 0; r < R; ++r) {
