@@ -37,6 +37,7 @@
  *   jr_engine_save / jr_engine_restore <- checkpoint of the whole engine (no reference API: sled persistence of
  *                         every node at once, chain.rs:119-123,198, plus the volatile State the reference loses)
  *   jr_truncate        <- no reference API (deviation D7)
+ *   jr_group_export / jr_group_import <- no reference API: reassigning a group to another engine
  *
  * One engine = G independent Raft groups x R replicas, all resident in one GPU's
  * HBM.  The reference is one group, one node per process; the group dimension is
@@ -655,6 +656,42 @@ jr_status jr_verify_groups(jr_engine* e, const uint32_t* groups, size_t n_groups
 jr_status jr_engine_save_size(jr_engine* e, size_t* bytes);
 jr_status jr_engine_save(jr_engine* e, void* buf, size_t cap);
 jr_status jr_engine_restore(jr_engine* e, const void* buf, size_t bytes);
+/*
+ * ---- moving groups between engines -------------------------------------------------------------------------------
+ * Group image: the complete state of some groups of one engine, in an opaque, versioned, checksummed byte format.
+ * Normative:
+ * jr_group_export(groups[0 .. n)):
+ *   Synchronous on the engine stream, ordered after everything already submitted.  *bytes = the image size; image == NULL
+ *   or cap < *bytes: JR_E_CAPACITY and the engine is untouched.  JR_E_INVAL, engine untouched, for a group out of range
+ *   or named twice.  A successful export DETACHES the groups: every replica of each is silenced (as jr_set_alive(.., 0)
+ *   leaves it), and its Instruction FIFO, fsm::Driver notification map and restart marks are emptied; its other planes
+ *   stay as they were, and the slot stays inert until an import overwrites it.  Detaching makes delivery exactly once: a
+ *   record an earlier jr_fsm_records_async already took leaves through that batch of the source; every record not yet
+ *   taken travels in the image and leaves through the destination's drains.  Export may run while record or leader-table
+ *   batches are outstanding.  A copy that leaves the source running is export followed by import into the same slots.
+ * jr_group_import(slots[0 .. n)), n = the number of groups in the image:
+ *   Group i of the image replaces whatever slot slots[i] held, that slot's undrained Instructions included.  It arrives
+ *   with, exactly as the source held them at export: every replica's P0-P3 and progress heads; its largest key, client
+ *   queue and stream digests / counts; its block-table window (floor and every present row); the mail in flight; its
+ *   record FIFO and counters; its notification map and restart marks; its jr_run_tokens route entry.  The source's and
+ *   the destination's mailbox parities may differ: the previous step's mail stays the previous step's mail.  From then on
+ *   the group steps exactly as it would have in the source, except for inputs keyed by the slot's global id: D2 draws use
+ *   (destination seed, destination group_offset + slot, node, draw#), draw# continuing from the carried count; synthetic
+ *   proposal tokens use the destination's step index and global id; jr_state_digest keys the group by its new global id.
+ *   Timers are absolute D1 milliseconds: the host drives both engines on one clock.
+ *   Everything is checked first; JR_E_INVAL, engine untouched, for: a bad magic or version, a checksum mismatch, a
+ *   truncated image, n other than the image's count, a slot out of range or named twice, or a configuration mismatch --
+ *   n_replicas, chain_capacity, mailbox_units, fsm_units, election_min_ms / max_ms, heartbeat_ms, resident_mask and flags
+ *   apart from JR_F_NO_SYMMETRIC_FOLD must match (seed, group_offset, n_groups, device, fsm_raw_units and fsm_host_records
+ *   may differ).  Every count in the image is checked on the host before anything reaches the device: mailbox units <=
+ *   mailbox_units, records <= fsm_units, notification runs <= JR_NOTIFY_RUNS, block ids ascending inside [floor, floor +
+ *   chain_capacity), ids, next and floor below 2^31 (mailbox units and records themselves are trusted as engine output,
+ *   under the checksum).  Synchronous.  Source and destination may be the same engine: moving groups between slots of one
+ *   engine is allowed.
+ */
+jr_status jr_group_export(jr_engine* e, const uint32_t* groups, size_t n, void* image, size_t cap, size_t* bytes);
+jr_status jr_group_import(jr_engine* e, const uint32_t* slots, size_t n, const void* image, size_t bytes);
+
 /* Silence the current leader of every group g with hash(seed,g,salt) % 1000 < permille. */
 jr_status jr_kill_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64_t* n_killed);
 

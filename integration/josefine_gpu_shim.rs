@@ -190,6 +190,10 @@ extern "C" {
     fn jr_node_restart_many(e: *mut c_void, now_ms: u64, chains: *const JrPersistedChain, n: usize, blocks: *const JrBlock,
                             n_blocks: usize) -> c_int;
     #[allow(dead_code)]
+    fn jr_group_export(e: *mut c_void, groups: *const u32, n: usize, image: *mut u8, cap: usize, bytes: *mut usize) -> c_int;
+    #[allow(dead_code)]
+    fn jr_group_import(e: *mut c_void, slots: *const u32, n: usize, image: *const u8, bytes: usize) -> c_int;
+    #[allow(dead_code)]
     fn jr_verify_groups(e: *mut c_void, groups: *const u32, n_groups: usize, report: *mut JrVerifyReport,
                         findings: *mut JrVerifyFinding, cap: usize, n_findings: *mut usize) -> c_int;
 }

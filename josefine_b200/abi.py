@@ -215,7 +215,7 @@ ENGINE_SYMBOLS = [
     "jr_chain_read", "jr_state_digest", "jr_stream_digest", "jr_fault_count", "jr_fold_count", "jr_compact",
     "jr_set_alive", "jr_kill_leaders", "jr_leader_table_device", "jr_leader_table", "jr_leader_table_async", "jr_leader_table_wait",
     "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_responses", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
-    "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_verify_groups", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
+    "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_verify_groups", "jr_group_export", "jr_group_import", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
 ]
 
 

@@ -1122,6 +1122,131 @@ __global__ void fsm_respond_kernel(const Dev d, const RespPlanes q, const FsmHea
   q.rd[i] = drop;
 }
 
+// ---- group export / import (jr_group_export / jr_group_import; the rules are normative in the ABI header) ------------
+// An image body holds, per (replica, listed group) in thread order t = (node - 1) * n + list index -- group-consecutive, so
+// a warp over consecutive groups reads each table row coalesced -- one fixed record of rec_units 16-byte units: the counts
+// {table rows, mailbox units, Instruction records, notification runs}, then the words of every plane the engine's plane
+// list (engine_planes, host side) carries word for word.  The variable parts follow, in the same order: the rows present
+// in the window as {id, next, token lo, token hi}, ascending id; the previous step's mailbox units; the records (2 units
+// each); the notification runs (2 units each).
+struct ImgPlane {
+  uint32_t* p;      // the plane, as 32-bit words
+  uint32_t words;   // words per entry
+  uint32_t depth;   // entries per replica (or group), one plane apart
+  uint32_t group;   // 1: one entry per group, indexed by the group (TB, the route); else per replica
+};
+
+__device__ __forceinline__ uint32_t img_var_units(uint4 c) { return c.x + c.y + 2u * c.z + 2u * c.w; }
+
+// Pass 1: thread t's counts -> cnt[t]; part[CTA] = the CTA's variable units (the host scans them).
+__global__ void group_count_kernel(const Dev d, const uint32_t* groups, uint32_t n, int prev, const uint32_t* pnc, uint4* cnt,
+                                   unsigned long long* part) {
+  __shared__ unsigned long long s[1][32];
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long v[1] = {0};
+  if (t < (size_t)d.R * n) {
+    const uint32_t r = (uint32_t)(t / n), g = groups[t % n];
+    const size_t plane = (size_t)d.R * d.Gp, i = (size_t)r * d.Gp + g;
+    const uint32_t floor = d.tb[g], span = window_span(d, i, floor);
+    uint32_t rows = 0;
+    for (uint32_t b = 0; b < span; ++b) rows += d.cnext[table_row(d, plane, floor + b, i)] != ABSENT ? 1u : 0u;
+    const uint32_t recs = (d.flags & JR_F_CAPTURE_FSM) ? min(d.fc[i].x, d.F) : 0u;
+    const uint4 c = make_uint4(rows, d.oc[prev][i], recs, pnc ? pnc[i] : 0u);
+    cnt[t] = c;
+    v[0] = img_var_units(c);
+  }
+  cta_sum(v, s);
+  if (threadIdx.x == 0) part[blockIdx.x] = v[0];
+}
+
+// Pass 2: thread t packs its fixed record and, at part[CTA] + the CTA-local scan, its variable part; then detaches the
+// replica: silenced, Instruction FIFO, notification map and restart marks empty.  Each thread reads and writes only its own
+// replica's column.
+__global__ void group_pack_kernel(const Dev d, const uint32_t* groups, uint32_t n, int prev, const ImgPlane* planes,
+                                  uint32_t n_planes, uint32_t rec_units, const uint4* cnt, const unsigned long long* part,
+                                  uint4* out, const RespPlanes q) {
+  __shared__ unsigned long long s_warp[32];
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool mine = t < (size_t)d.R * n;
+  const uint4 c = mine ? cnt[t] : make_uint4(0u, 0u, 0u, 0u);
+  const unsigned long long at = part[blockIdx.x] + cta_exclusive_scan((unsigned long long)img_var_units(c), s_warp);
+  if (!mine) return;
+  const uint32_t r = (uint32_t)(t / n), g = groups[t % n];
+  const size_t plane = (size_t)d.R * d.Gp, i = (size_t)r * d.Gp + g;
+  uint4* rec = out + t * rec_units;
+  rec[0] = c;
+  uint32_t* w = reinterpret_cast<uint32_t*>(rec + 1);
+  for (uint32_t k = 0; k < n_planes; ++k) {
+    const ImgPlane pl = planes[k];
+    const size_t at_p = pl.group ? g : i, stride = pl.group ? d.Gp : plane;
+    for (uint32_t e = 0; e < pl.depth; ++e)
+      for (uint32_t x = 0; x < pl.words; ++x) *w++ = pl.p[((size_t)e * stride + at_p) * pl.words + x];
+  }
+  uint4* v = out + (size_t)d.R * n * rec_units + at;
+  const uint32_t floor = d.tb[g], span = window_span(d, i, floor);
+  for (uint32_t b = 0, k = 0; b < span && k < c.x; ++b) {
+    const size_t row = table_row(d, plane, floor + b, i);
+    const uint32_t nx = d.cnext[row];
+    if (nx == ABSENT) continue;
+    const unsigned long long tok = d.ctok[row];
+    *v++ = make_uint4(floor + b, nx, (uint32_t)tok, (uint32_t)(tok >> 32));
+    ++k;
+  }
+  for (uint32_t u = 0; u < c.y; ++u) *v++ = d.ob[prev][(size_t)u * plane + i];
+  for (uint32_t k = 0; k < 2u * c.z; ++k) *v++ = d.fs[(size_t)k * plane + i];
+  for (uint32_t k = 0; k < 2u * c.w; ++k) *v++ = q.pn[(size_t)k * plane + i];
+  d.p2[i].w = d.p2[i].w | META_DEAD;
+  d.fc[i] = make_uint2(0u, 0u);
+  if (q.pnc) {
+    q.pnc[i] = 0u;
+    q.rm[i] = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
+// Import: one thread per listed group j, into slot slots[j].  Host-validated: distinct slots; counts within the engine's
+// limits; rows ascending inside [floor, floor + cap).  The old occupant's rows are only its window_span (truncation keeps
+// every other row absent): those are cleared first, then the carried rows, planes, mail, records and runs are written.
+// Records carry their group: it becomes the slot.
+__global__ void group_unpack_kernel(const Dev d, const uint32_t* slots, uint32_t n, int prev, const ImgPlane* planes,
+                                    uint32_t n_planes, uint32_t rec_units, const uint4* img, const unsigned long long* off,
+                                    const RespPlanes q) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t g = slots[j];
+  const size_t plane = (size_t)d.R * d.Gp;
+  const uint32_t old_floor = d.tb[g];
+  const uint4* var0 = img + (size_t)d.R * n * rec_units;
+  for (uint32_t r = 0; r < d.R; ++r) {
+    const size_t t = (size_t)r * n + j, i = (size_t)r * d.Gp + g;
+    for (uint32_t b = window_span(d, i, old_floor); b-- > 0;) d.cnext[table_row(d, plane, old_floor + b, i)] = ABSENT;
+    const uint4* rec = img + t * rec_units;
+    const uint4 c = rec[0];
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(rec + 1);
+    for (uint32_t k = 0; k < n_planes; ++k) {
+      const ImgPlane pl = planes[k];
+      if (pl.group && r != 0) { w += pl.depth * pl.words; continue; }   // a group's words are taken from its first replica
+      const size_t at_p = pl.group ? g : i, stride = pl.group ? d.Gp : plane;
+      for (uint32_t e = 0; e < pl.depth; ++e)
+        for (uint32_t x = 0; x < pl.words; ++x) pl.p[((size_t)e * stride + at_p) * pl.words + x] = *w++;
+    }
+    const uint4* v = var0 + off[t];
+    for (uint32_t k = 0; k < c.x; ++k, ++v) {
+      const size_t row = table_row(d, plane, v->x, i);
+      d.cnext[row] = v->y;
+      d.ctok[row] = (unsigned long long)v->z | ((unsigned long long)v->w << 32);
+    }
+    for (uint32_t u = 0; u < c.y; ++u) d.ob[prev][(size_t)u * plane + i] = *v++;
+    d.oc[prev][i] = c.y;
+    for (uint32_t k = 0; k < c.z; ++k) {
+      uint4 h = *v++;
+      h.x = g;
+      d.fs[(size_t)(2 * k) * plane + i] = h;
+      d.fs[(size_t)(2 * k + 1) * plane + i] = *v++;
+    }
+    for (uint32_t k = 0; k < 2u * c.w; ++k) q.pn[(size_t)k * plane + i] = *v++;
+  }
+}
+
 __global__ void max_u32_kernel(const uint32_t* v, size_t n, uint32_t* out) {
   __shared__ uint32_t s[1][32];
   uint32_t m[1] = {0};
@@ -1203,6 +1328,12 @@ struct jr_engine {
   // scratch of jr_verify_groups (device, grows; not part of a checkpoint): report, CTA offsets, group list, verdicts
   void* verify_buf = nullptr;
   size_t verify_cap = 0;
+  // scratch of jr_group_export / jr_group_import (device, grows; not part of a checkpoint): list, plane list, counts and
+  // CTA offsets in move_buf, the image body in move_img
+  void* move_buf = nullptr;
+  size_t move_cap = 0;
+  void* move_img = nullptr;
+  size_t move_img_cap = 0;
   // Instruction-stream drain (JR_F_CAPTURE_FSM): scan -> pack into stage[b] on the engine stream, then
   // the copy engine moves stage[b] into the pinned host buffer host[b] on the d2h stream.
   // One slot more than batches may be outstanding, used round robin: with NBUF batches outstanding at a
@@ -1670,6 +1801,8 @@ void jr_engine_destroy(jr_engine* e) {
   if (e->inj_targets) cudaFree(e->inj_targets);
   if (e->many_buf) cudaFree(e->many_buf);
   if (e->verify_buf) cudaFree(e->verify_buf);
+  if (e->move_buf) cudaFree(e->move_buf);
+  if (e->move_img) cudaFree(e->move_img);
   if (e->h2d) { cudaStreamSynchronize(e->h2d); cudaStreamDestroy(e->h2d); }
   if (e->d2h) { cudaStreamSynchronize(e->d2h); cudaStreamDestroy(e->d2h); }
   for (int i = 0; i < jr_engine::NBUF; ++i) {
@@ -2920,22 +3053,54 @@ struct SaveHeader {
   uint64_t step_index;
 };
 constexpr uint64_t SAVE_MAGIC = 0x4a52454e47494e32ull;  // "JRENGIN2"
-struct Segment { void* p; size_t n; };
-std::vector<Segment> save_segments(jr_engine* e) {
+// Every allocation that holds the state of a group, in checkpoint order, and how a group image carries its share of it.
+// jr_engine_save writes each one whole; jr_group_export carries each listed group's part of each one.  (The allocations
+// that are neither -- transient scratch and engine-wide state -- are listed in DESIGN.md section 3f.)
+enum class Carry : uint8_t {
+  WORDS,        // word for word in the fixed record: per replica, or per group (per_group)
+  TABLE,        // cnext / ctok: the rows present in the window
+  MAIL,         // ob[0..1] / oc[0..1]: the previous step's mailbox, moved to the destination's parity
+  FIFO,         // fs: the records fc counts
+  NOTIFY_RUNS,  // the PN runs pnc counts
+};
+struct PlaneDesc {
+  void* p;
+  size_t bytes;                    // the checkpoint segment
+  Carry carry;
+  uint32_t words = 0, depth = 1;   // WORDS: 32-bit words per entry, entries per replica / group
+  bool per_group = false;
+};
+std::vector<PlaneDesc> engine_planes(jr_engine* e) {
   const Dev& d = e->d;
   const size_t plane = (size_t)d.R * d.Gp;
   const size_t rows = (size_t)d.capm + 1;
-  std::vector<Segment> v = {
-      {d.p0, plane * sizeof(uint4)}, {d.p1, plane * sizeof(uint4)}, {d.p2, plane * sizeof(uint4)}, {d.p3, plane * sizeof(uint4)},
-      {d.pr, plane * ((d.R + 3) / 4) * sizeof(uint4)}, {d.mk, plane * sizeof(uint32_t)},
-      {d.qt, plane * JR_CLIENT_QUEUE_CAP * sizeof(uint4)}, {d.dg, plane * sizeof(uint4)}, {d.cn, plane * sizeof(uint2)},
-      {d.cnext, plane * rows * sizeof(uint32_t)}, {d.ctok, plane * rows * sizeof(unsigned long long)},
-      {d.ob[0], plane * (size_t)d.U * sizeof(uint4)}, {d.ob[1], plane * (size_t)d.U * sizeof(uint4)},
-      {d.oc[0], plane * sizeof(uint32_t)}, {d.oc[1], plane * sizeof(uint32_t)},
-      {d.fs, plane * ((d.flags & JR_F_CAPTURE_FSM) ? 2 * (size_t)d.F : 1) * sizeof(uint4)}, {d.fc, plane * sizeof(uint2)},
-      {d.tb, (size_t)d.Gp * sizeof(uint32_t)}, {e->route, (size_t)d.G * sizeof(uint32_t)}};
-  if (e->rp.pn)   // the fsm::Driver maps (JR_F_CLIENT_RESPONSES only: other checkpoints keep their size and bytes)
-    v.push_back({e->rp.pn, pn_units(plane) * sizeof(uint4)});
+  const uint32_t pq = (d.R + 3) / 4;
+  std::vector<PlaneDesc> v = {
+      {d.p0, plane * sizeof(uint4), Carry::WORDS, 4}, {d.p1, plane * sizeof(uint4), Carry::WORDS, 4},
+      {d.p2, plane * sizeof(uint4), Carry::WORDS, 4}, {d.p3, plane * sizeof(uint4), Carry::WORDS, 4},
+      {d.pr, plane * pq * sizeof(uint4), Carry::WORDS, 4, pq}, {d.mk, plane * sizeof(uint32_t), Carry::WORDS, 1},
+      {d.qt, plane * JR_CLIENT_QUEUE_CAP * sizeof(uint4), Carry::WORDS, 4, JR_CLIENT_QUEUE_CAP},
+      {d.dg, plane * sizeof(uint4), Carry::WORDS, 4}, {d.cn, plane * sizeof(uint2), Carry::WORDS, 2},
+      {d.cnext, plane * rows * sizeof(uint32_t), Carry::TABLE}, {d.ctok, plane * rows * sizeof(unsigned long long), Carry::TABLE},
+      {d.ob[0], plane * (size_t)d.U * sizeof(uint4), Carry::MAIL}, {d.ob[1], plane * (size_t)d.U * sizeof(uint4), Carry::MAIL},
+      {d.oc[0], plane * sizeof(uint32_t), Carry::MAIL}, {d.oc[1], plane * sizeof(uint32_t), Carry::MAIL},
+      {d.fs, plane * ((d.flags & JR_F_CAPTURE_FSM) ? 2 * (size_t)d.F : 1) * sizeof(uint4), Carry::FIFO},
+      {d.fc, plane * sizeof(uint2), Carry::WORDS, 2},
+      {d.tb, (size_t)d.Gp * sizeof(uint32_t), Carry::WORDS, 1, 1, true},
+      {e->route, (size_t)d.G * sizeof(uint32_t), Carry::WORDS, 1, 1, true}};
+  if (e->rp.pn) {   // the fsm::Driver maps (JR_F_CLIENT_RESPONSES only: other checkpoints keep their size and bytes)
+    // one allocation, three consecutive segments: runs, run counts (u32, padded to 16 bytes), restart marks
+    v.push_back({e->rp.pn, 2 * (size_t)JR_NOTIFY_RUNS * plane * sizeof(uint4), Carry::NOTIFY_RUNS});
+    v.push_back({e->rp.pnc, (plane + 3) / 4 * sizeof(uint4), Carry::WORDS, 1});
+    v.push_back({e->rp.rm, plane * sizeof(uint4), Carry::WORDS, 4});
+  }
+  return v;
+}
+
+struct Segment { void* p; size_t n; };
+std::vector<Segment> save_segments(jr_engine* e) {
+  std::vector<Segment> v;
+  for (const PlaneDesc& pd : engine_planes(e)) v.push_back({pd.p, pd.bytes});
   return v;
 }
 }  // namespace
@@ -2998,6 +3163,226 @@ jr_status jr_engine_restore(jr_engine* e, const void* buf, size_t bytes) {
   e->step_index = h.step_index;
   e->fsm_npending = 0;
   e->resp_b = -1;
+  return JR_OK;
+}
+
+// ---- group export / import ---------------------------------------------------------------------------------------------
+namespace {
+struct ImageHeader {
+  uint64_t magic;
+  uint32_t version, n_groups;
+  uint64_t bytes, checksum;      // the whole image; the checksum is taken with this field zero
+  jr_config cfg;                 // the source's
+  uint32_t rec_units, words;     // fixed record size and the words of its planes: a different plane list is refused
+  uint32_t reserved[4];
+};
+static_assert(sizeof(ImageHeader) % 16 == 0, "the image body starts 16-byte aligned");
+constexpr uint64_t IMAGE_MAGIC = 0x4a5247524f555031ull;   // "JRGROUP1"
+constexpr uint32_t IMAGE_VERSION = 1;
+
+struct ImgLayout {
+  std::vector<ImgPlane> planes;   // the WORDS planes, in list order
+  uint32_t words = 0, rec_units = 0;
+  uint32_t w_fc = 0, w_tb = 0, w_pnc = ~0u;   // word offsets inside a record's planes
+};
+ImgLayout img_layout(jr_engine* e) {
+  ImgLayout L;
+  for (const PlaneDesc& pd : engine_planes(e)) {
+    if (pd.carry != Carry::WORDS) continue;
+    if (pd.p == e->d.fc) L.w_fc = L.words;
+    if (pd.p == e->d.tb) L.w_tb = L.words;
+    if (pd.p == e->rp.pnc) L.w_pnc = L.words;
+    L.planes.push_back(ImgPlane{(uint32_t*)pd.p, pd.words, pd.depth, pd.per_group ? 1u : 0u});
+    L.words += pd.words * pd.depth;
+  }
+  L.rec_units = 1 + (L.words + 3) / 4;
+  return L;
+}
+
+// Fields two engines must share for an image of one to run in the other (JR_F_NO_SYMMETRIC_FOLD only picks a code path).
+bool image_config_matches(const jr_config& a, const jr_config& b) {
+  const uint32_t keep = ~(uint32_t)JR_F_NO_SYMMETRIC_FOLD;
+  return a.abi_version == b.abi_version && a.n_replicas == b.n_replicas && a.chain_capacity == b.chain_capacity &&
+         a.mailbox_units == b.mailbox_units && a.fsm_units == b.fsm_units && a.election_min_ms == b.election_min_ms &&
+         a.election_max_ms == b.election_max_ms && a.heartbeat_ms == b.heartbeat_ms && a.resident_mask == b.resident_mask &&
+         (a.flags & keep) == (b.flags & keep);
+}
+
+// Four independent multiply-rotate lanes over 8-byte words, folded with mix64: a damaged byte anywhere changes it.
+uint64_t image_checksum(const unsigned char* p, size_t n) {
+  uint64_t h[4] = {0x243f6a8885a308d3ull, 0x13198a2e03707344ull, 0xa4093822299f31d0ull, 0x082efa98ec4e6c89ull};
+  auto lane = [](uint64_t x, uint64_t w) {
+    x ^= w * 0x9e3779b97f4a7c15ull;
+    return ((x << 31) | (x >> 33)) * 0xbf58476d1ce4e5b9ull;
+  };
+  size_t k = 0;
+  for (; k + 32 <= n; k += 32)
+    for (int l = 0; l < 4; ++l) {
+      uint64_t w;
+      memcpy(&w, p + k + 8 * l, 8);
+      h[l] = lane(h[l], w);
+    }
+  uint64_t tail = 0;
+  for (size_t b = 0; k + b < n; ++b) tail = mix64(tail ^ ((uint64_t)p[k + b] << 8 | b));
+  return mix64(mix64(mix64(mix64(h[0] ^ n) ^ h[1]) ^ h[2]) ^ h[3] ^ mix64(tail + (n - k)));
+}
+
+uint64_t header_checksum(const unsigned char* image, size_t bytes) {
+  ImageHeader h;
+  memcpy(&h, image, sizeof h);
+  h.checksum = 0;
+  const uint64_t a = image_checksum(reinterpret_cast<const unsigned char*>(&h), sizeof h);
+  return mix64(a ^ image_checksum(image + sizeof h, bytes - sizeof h));
+}
+
+inline size_t up16(size_t b) { return (b + 15) / 16 * 16; }
+}  // namespace
+
+jr_status jr_group_export(jr_engine* e, const uint32_t* groups, size_t n, void* image, size_t cap, size_t* bytes) {
+  if (!e || !bytes || (n && !groups)) return JR_E_INVAL;
+  const Dev& d = e->d;
+  if (n > d.G) { set_err("more groups than the engine holds"); return JR_E_INVAL; }
+  {   // checked before the first device call: on JR_E_INVAL the engine is untouched
+    std::vector<uint8_t> seen(d.G, 0);
+    for (size_t k = 0; k < n; ++k) {
+      if (groups[k] >= d.G || seen[groups[k]]) {
+        set_err("groups[%zu]: out of range or named twice", k);
+        return JR_E_INVAL;
+      }
+      seen[groups[k]] = 1;
+    }
+  }
+  CK(cudaSetDevice(e->cfg.device));
+  const ImgLayout L = img_layout(e);
+  const uint32_t T = CTA_THREADS;
+  const size_t reps = (size_t)d.R * n;
+  const uint32_t n_ctas = (uint32_t)((reps + T - 1) / T);
+  const size_t o_planes = up16(n * sizeof(uint32_t)), o_part = o_planes + up16(L.planes.size() * sizeof(ImgPlane));
+  const size_t o_cnt = o_part + up16((size_t)n_ctas * sizeof(unsigned long long));
+  jr_status st = scratch_reserve(&e->move_buf, &e->move_cap, o_cnt + reps * sizeof(uint4));
+  if (st != JR_OK) return st;
+  char* base = (char*)e->move_buf;
+  const uint32_t* dgroups = (const uint32_t*)base;
+  const ImgPlane* dplanes = (const ImgPlane*)(base + o_planes);
+  unsigned long long* dpart = (unsigned long long*)(base + o_part);
+  uint4* dcnt = (uint4*)(base + o_cnt);
+  const int prev = e->cur ^ 1;   // the mailbox the previous step wrote: the mail in flight
+  std::vector<unsigned long long> part(n_ctas);
+  if (reps) {
+    CK(cudaMemcpyAsync(base, groups, n * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(base + o_planes, L.planes.data(), L.planes.size() * sizeof(ImgPlane), cudaMemcpyHostToDevice, e->stream));
+    JR_LAUNCH(group_count_kernel, n_ctas, T, e->stream, d, dgroups, (uint32_t)n, prev, (const uint32_t*)e->rp.pnc, dcnt, dpart);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(part.data(), dpart, n_ctas * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
+  }
+  CK(cudaStreamSynchronize(e->stream));   // (also covers `groups` and the plane list)
+  unsigned long long var = 0;
+  for (uint32_t k = 0; k < n_ctas; ++k) { const unsigned long long v = part[k]; part[k] = var; var += v; }
+  const size_t body = (reps * L.rec_units + (size_t)var) * sizeof(uint4);
+  *bytes = sizeof(ImageHeader) + body;
+  if (!image || cap < *bytes) { set_err("the image needs %zu bytes", *bytes); return JR_E_CAPACITY; }
+  if (reps) {
+    if ((st = scratch_reserve(&e->move_img, &e->move_img_cap, body)) != JR_OK) return st;
+    CK(cudaMemcpyAsync(dpart, part.data(), n_ctas * sizeof(unsigned long long), cudaMemcpyHostToDevice, e->stream));
+    JR_LAUNCH(group_pack_kernel, n_ctas, T, e->stream, d, dgroups, (uint32_t)n, prev, dplanes, (uint32_t)L.planes.size(),
+              L.rec_units, (const uint4*)dcnt, (const unsigned long long*)dpart, (uint4*)e->move_img, e->rp);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync((char*)image + sizeof(ImageHeader), e->move_img, body, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  ImageHeader h;
+  memset(&h, 0, sizeof h);
+  h.magic = IMAGE_MAGIC;
+  h.version = IMAGE_VERSION;
+  h.n_groups = (uint32_t)n;
+  h.bytes = *bytes;
+  h.cfg = e->cfg;
+  h.rec_units = L.rec_units;
+  h.words = L.words;
+  memcpy(image, &h, sizeof h);
+  h.checksum = header_checksum((const unsigned char*)image, *bytes);
+  memcpy(image, &h, sizeof h);
+  return JR_OK;
+}
+
+jr_status jr_group_import(jr_engine* e, const uint32_t* slots, size_t n, const void* image, size_t bytes) {
+  if (!e || (n && !slots) || !image) return JR_E_INVAL;
+  const Dev& d = e->d;
+  // everything is checked before the first device write: on JR_E_INVAL the engine is untouched
+  ImageHeader h;
+  if (bytes < sizeof h) { set_err("truncated image"); return JR_E_INVAL; }
+  memcpy(&h, image, sizeof h);
+  const unsigned char* img = (const unsigned char*)image;
+  if (h.magic != IMAGE_MAGIC || h.version != IMAGE_VERSION) { set_err("not a group image of this version"); return JR_E_INVAL; }
+  if (h.bytes > bytes || h.bytes < sizeof h) { set_err("truncated image"); return JR_E_INVAL; }
+  if (header_checksum(img, h.bytes) != h.checksum) { set_err("image checksum mismatch"); return JR_E_INVAL; }
+  if (h.n_groups != n) { set_err("the image holds %u groups, %zu slots given", h.n_groups, n); return JR_E_INVAL; }
+  {
+    std::vector<uint8_t> seen(d.G, 0);
+    for (size_t k = 0; k < n; ++k) {
+      if (slots[k] >= d.G || seen[slots[k]]) {
+        set_err("slots[%zu]: out of range or named twice", k);
+        return JR_E_INVAL;
+      }
+      seen[slots[k]] = 1;
+    }
+  }
+  if (!image_config_matches(h.cfg, e->cfg)) { set_err("the image's engine configuration does not match this engine's"); return JR_E_INVAL; }
+  const ImgLayout L = img_layout(e);
+  if (h.rec_units != L.rec_units || h.words != L.words) { set_err("the image's record layout does not match"); return JR_E_INVAL; }
+  const size_t reps = (size_t)d.R * n, fixed = reps * L.rec_units;
+  const size_t body = (size_t)h.bytes - sizeof h;
+  if (body % sizeof(uint4) || body / sizeof(uint4) < fixed) { set_err("truncated image"); return JR_E_INVAL; }
+  const size_t units = body / sizeof(uint4);
+  auto unit = [&](size_t u) { uint4 v; memcpy(&v, img + sizeof h + u * sizeof(uint4), sizeof v); return v; };
+  auto word = [&](size_t t, uint32_t w) { uint32_t v; memcpy(&v, img + sizeof h + (t * L.rec_units + 1) * sizeof(uint4) + 4 * (size_t)w, 4); return v; };
+  std::vector<unsigned long long> off(reps);
+  std::vector<uint32_t> floor(n);
+  unsigned long long at = 0;
+  for (size_t t = 0; t < reps; ++t) {   // counts, first
+    const size_t j = t % n;
+    const uint4 c = unit(t * L.rec_units);
+    const uint32_t fcx = word(t, L.w_fc), fl = word(t, L.w_tb);
+    const bool capture = (d.flags & JR_F_CAPTURE_FSM) != 0;
+    if (c.x > d.cap || c.y > d.U || c.z > (capture ? d.F : 0u) || c.z != std::min(fcx, capture ? d.F : 0u) ||
+        c.w > (e->rp.pn ? JR_NOTIFY_RUNS : 0u) || (L.w_pnc != ~0u && word(t, L.w_pnc) != c.w)) {
+      set_err("record %zu: counts outside the engine's limits", t);
+      return JR_E_INVAL;
+    }
+    if (t < n) floor[j] = fl;
+    if (fl >= JR_BLOCK_ID_LIMIT || fl != floor[j]) { set_err("record %zu: floor >= 2^31 or not the group's", t); return JR_E_INVAL; }
+    off[t] = at;
+    at += (unsigned long long)c.x + c.y + 2ull * c.z + 2ull * c.w;
+  }
+  if (fixed + at != units) { set_err("truncated image"); return JR_E_INVAL; }
+  for (size_t t = 0; t < reps; ++t) {   // then the rows: ascending, inside the window, below 2^31 (D4, D7)
+    const uint32_t rows = unit(t * L.rec_units).x;
+    const uint64_t lo = floor[t % n];
+    for (uint32_t k = 0; k < rows; ++k) {
+      const uint4 b = unit(fixed + off[t] + k);
+      if (b.x < lo || b.x - lo >= d.cap || b.x >= JR_BLOCK_ID_LIMIT || b.y >= JR_BLOCK_ID_LIMIT ||
+          (k && b.x <= unit(fixed + off[t] + k - 1).x)) {
+        set_err("record %zu row %u: id not ascending, outside [floor, floor + chain_capacity) or >= 2^31, or next >= 2^31", t, k);
+        return JR_E_INVAL;
+      }
+    }
+  }
+  if (n == 0) return JR_OK;
+  CK(cudaSetDevice(e->cfg.device));
+  const size_t o_planes = up16(n * sizeof(uint32_t)), o_off = o_planes + up16(L.planes.size() * sizeof(ImgPlane));
+  jr_status st = scratch_reserve(&e->move_buf, &e->move_cap, o_off + reps * sizeof(unsigned long long));
+  if (st != JR_OK) return st;
+  if ((st = scratch_reserve(&e->move_img, &e->move_img_cap, body)) != JR_OK) return st;
+  char* base = (char*)e->move_buf;
+  CK(cudaMemcpyAsync(base, slots, n * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(base + o_planes, L.planes.data(), L.planes.size() * sizeof(ImgPlane), cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(base + o_off, off.data(), reps * sizeof(unsigned long long), cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(e->move_img, img + sizeof h, body, cudaMemcpyHostToDevice, e->stream));
+  JR_LAUNCH(group_unpack_kernel, (unsigned)((n + 127) / 128), 128, e->stream, d, (const uint32_t*)base, (uint32_t)n, e->cur ^ 1,
+            (const ImgPlane*)(base + o_planes), (uint32_t)L.planes.size(), L.rec_units, (const uint4*)e->move_img,
+            (const unsigned long long*)(base + o_off), e->rp);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(e->stream));
   return JR_OK;
 }
 

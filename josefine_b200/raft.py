@@ -498,6 +498,27 @@ class RaftApi:
         self._check(fn(self._h, gs, C.c_size_t(n), C.byref(rep), buf, need, C.byref(need)), "verify_groups")
         return rep, [buf[i] for i in range(need.value)]
 
+    def export_groups(self, groups: Sequence[int]) -> bytes:
+        """jr_group_export: the image of `groups` (sized, then exported).  The groups are detached from this engine."""
+        groups = list(groups)
+        n = len(groups)
+        gs = (C.c_uint32 * max(n, 1))(*groups)
+        need = C.c_size_t(0)
+        fn = self._fn("group_export")
+        st = fn(self._h, gs, C.c_size_t(n), None, C.c_size_t(0), C.byref(need))
+        if st != abi.E_CAPACITY:
+            self._check(st, "group_export")
+        buf = C.create_string_buffer(need.value)
+        self._check(fn(self._h, gs, C.c_size_t(n), buf, need, C.byref(need)), "group_export")
+        return buf.raw
+
+    def import_groups(self, slots: Sequence[int], image: bytes):
+        """jr_group_import: group i of `image` replaces slot slots[i]."""
+        slots = list(slots)
+        ss = (C.c_uint32 * max(len(slots), 1))(*slots)
+        buf = C.create_string_buffer(image, len(image))
+        self._check(self._fn("group_import")(self._h, ss, C.c_size_t(len(slots)), buf, C.c_size_t(len(image))), "group_import")
+
     def save(self) -> bytes:
         """jr_engine_save: checkpoint of everything the engine holds."""
         n = C.c_size_t(0)
@@ -591,6 +612,8 @@ def _bind(lib: C.CDLL, p: str):
         "node_restart_many": [vp, C.c_uint64, C.POINTER(abi.PersistedChain), C.c_size_t, C.POINTER(abi.Block), C.c_size_t],
         "verify_groups": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(abi.VerifyReport), C.POINTER(abi.VerifyFinding),
                           C.c_size_t, C.POINTER(C.c_size_t)],
+        "group_export": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)],
+        "group_import": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.c_void_p, C.c_size_t],
         "engine_save_size": [vp, C.POINTER(C.c_size_t)],
         "engine_save": [vp, C.c_void_p, C.c_size_t],
         "engine_restore": [vp, C.c_void_p, C.c_size_t],
