@@ -1467,14 +1467,14 @@ template <int R>
 static void launch_sym_r(jr_engine* e, const StepParams& p) {
   if constexpr (R >= 2) {
     // the entry checks, then the fold that consumes their records: nothing may run between the two
-    JR_LAUNCH(sym_check_kernel<R>, (e->d.Gp + SYM_CHECK_THREADS - 1) / SYM_CHECK_THREADS, SYM_CHECK_THREADS, e->stream, e->d, p,
-              e->symrec);
+    JR_LAUNCH_SMEM(sym_check_kernel<R>, e->d.Gp / 32, 32 * R, sym_check_smem_words(R) * sizeof(uint32_t), e->stream, e->d, p,
+                   e->symrec);
     JR_LAUNCH_SMEM(sym2_kernel<R>, (e->d.Gp + SYM2_GROUPS - 1) / SYM2_GROUPS, 2 * SYM2_GROUPS,
                    (size_t)SYM2_UNITS * SYM2_GROUPS * sizeof(uint4), e->stream, e->d, p, e->symdone, e->symblk, e->symrec);
   }
 }
 
-// May this launch be offered to the symmetric-group fold?  (Whether a GROUP takes it is sym_enter's decision.)
+// May this launch be offered to the symmetric-group fold?  (Whether a GROUP takes it is sym_check_kernel's decision.)
 static bool fold_eligible(const jr_engine* e, const StepParams& p) {
   const Dev& d = e->d;
   const uint32_t whole = PH_RESET_OUT | PH_DRAIN | PH_TICK;

@@ -14,7 +14,7 @@
 // Exactness contract:
 //   * sym_check_kernel, launched right before sym2_kernel with nothing in between, FIRST CHECKS that a group is
 //     symmetric, that its followers' tables agree over every id the launch can read, and that its mail in flight has the
-//     canonical shapes (sym_enter), on the planes the fold is about to read; every other group is left to step_kernel
+//     canonical shapes, on the planes the fold is about to read; every other group is left to step_kernel
 //     untouched.  The fold takes the verdict and its starting state from the entry record the check leaves behind.
 //   * If anything outside the canonical evolution would happen during the launch (a fault, an election timer that
 //     could fire, a HeartbeatResponse{has_committed: false}, a read below the compared rows, ...) the lane ABORTS (it
@@ -82,8 +82,8 @@ constexpr uint32_t SYM_SMEM_UNITS = 2 * SYM_ROWS + SYM_ENC_L + SYM_ENC_F;   // u
 // latency bound with 3.5 warps per SM sub-partition; two double the warps and halve each warp's serial chain.  The mail goes
 // through shared memory, double buffered, one __syncthreads() per tick:
 //   leader -> followers   A = {hb | ae << 1 | nb << 4 | abort << 8 | ids << 9 | mode << 10, commit, leader's max key, id0 / progress head}
-//                         B = {id1 .. id4}   (ids = 1: the AppendEntries' blocks are listed -- the mail sym_enter found in
-//                         flight; ids = 0: the follower lane derives them, see replicate())
+//                         B = {id1 .. id4}   (ids = 1: the AppendEntries' blocks are listed -- the mail sym_check_kernel found
+//                         in flight; ids = 0: the follower lane derives them, see replicate())
 //   followers -> leader   C = {hbr | has << 1 | ar << 2 | abort << 8, hbr_commit, ar_head, -}
 constexpr uint32_t SYM2_GROUPS = 64;                                        // groups per CTA: 128 threads
 constexpr uint32_t SYM2_UNITS = SYM_SMEM_UNITS + 2 * 2 + 2 * 1;            // uint4 per group
@@ -125,8 +125,7 @@ enum : uint32_t {
 #define JR_SYM_ABORT(s, site) ((s).abort = true)
 #endif
 
-// CHECK: the group as sym_check_kernel sees it -- no row caches, every table read goes to global memory.
-template <int R, bool CHECK = false>
+template <int R>
 struct SymGroup {
   static constexpr uint32_t STRIDE = SYM2_GROUPS;   // columns of the CTA's per-group shared memory
   const Dev& d;
@@ -140,7 +139,7 @@ struct SymGroup {
   uint32_t n_hb;                           // heartbeats the followers took in this launch
   uint64_t last_hb;
   uint32_t tbase;
-  uint32_t flo;                            // lowest id whose row sym_enter found identical in every follower
+  uint32_t flo;                            // lowest id whose row sym_check_kernel found identical in every follower
   uint4* rows;                             // this lane's column of the CTA's row caches (see above)
   uint4* enc;                              // this lane's column of the encoder states (see above)
   uint32_t lcnt, fcnt;                     // raw Instructions emitted: leader / each follower
@@ -180,7 +179,7 @@ struct SymGroup {
   }
   __device__ __forceinline__ size_t rg(uint32_t r) const { return (size_t)r * d.Gp + g; }
   __device__ __forceinline__ size_t row(uint32_t r, uint32_t bid) const { return table_row(d, plane, bid, rg(r)); }
-  __device__ __forceinline__ bool in_window(uint32_t bid) const { return bid - tbase < d.cap; }   // (sym_enter made sure ids stay below 2^31)
+  __device__ __forceinline__ bool in_window(uint32_t bid) const { return bid - tbase < d.cap; }   // (sym_check_kernel made sure ids stay below 2^31)
   __device__ __forceinline__ uint4& slot(uint32_t r, uint32_t bid) const { return rows[((r == L ? 0u : SYM_ROWS) + (bid % SYM_ROWS)) * STRIDE]; }
   __device__ __forceinline__ void cache_put(uint32_t r, uint32_t bid, uint32_t nx, uint64_t tk) const {
     slot(r, bid) = make_uint4(bid, nx, (uint32_t)tk, (uint32_t)(tk >> 32));
@@ -188,7 +187,6 @@ struct SymGroup {
   // r is the leader (its own table) or F0 (the followers' table)
   __device__ __forceinline__ void fetch(uint32_t r, uint32_t bid, uint32_t& next, uint64_t& tok) {
     if (!in_window(bid)) { next = ABSENT; tok = 0; return; }
-    if (CHECK) { next = d.cnext[row(r, bid)]; tok = d.ctok[row(r, bid)]; return; }
     const uint4 e = slot(r, bid);
     if (e.x == bid) { next = e.y; tok = (uint64_t)e.z | ((uint64_t)e.w << 32); return; }
     next = __ldcg(d.cnext + row(r, bid));   // rows written earlier in this launch by this lane: read them at L2
@@ -230,7 +228,7 @@ struct SymGroup {
     fetch(r, bid, n, t);
     return n != ABSENT;
   }
-  // The followers' table, read through the lowest follower's: only rows sym_enter compared across followers (>= flo),
+  // The followers' table, read through the lowest follower's: only rows sym_check_kernel compared across followers (>= flo),
   // rows this launch wrote to all of them, or ids below the floor (absent everywhere) may be answered that way.
   __device__ __forceinline__ void fetch_f(uint32_t bid, uint32_t& next, uint64_t& tok) {
     if (in_window(bid) && bid < flo) { JR_SYM_ABORT(*this, SA_FETCH_F); next = ABSENT; tok = 0; return; }
@@ -521,7 +519,7 @@ struct SymGroup {
         out.ar_head = fhead;
       }
     }
-    // Command::Tick: the election timer cannot have expired (sym_enter checked the bound)
+    // Command::Tick: the election timer cannot have expired (sym_check_kernel checked the bound)
   }
   // sym2_kernel, follower lane: the same tick when the AppendEntries' blocks are not listed in the mail.  The leader's
   // replicate() (leader.rs:124-174: Probe -> range(head..).nth(1); Replicate -> range(head..).skip(1).take(5)) is run
@@ -556,215 +554,11 @@ struct SymGroup {
   }
 };
 
-// ---- entry: is the group symmetric, is its mail canonical? (run by sym_check_kernel, below) ---------------------------
-template <int R>
-__device__ __forceinline__ bool sym_enter(SymGroup<R, true>& s, SymMail& m, const StepParams& p, int prv) {
-  const Dev& d = s.d;
-  if (s.g >= d.G) return false;
-  // roles: one live leader, R-1 live followers of that leader
-  uint32_t L = R, nlead = 0;
-  uint4 p2[R];
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    p2[r] = d.p2[s.rg(r)];
-    const uint32_t meta = p2[r].w;
-    if (!meta_live(meta)) return false;                                       // faulted or silenced
-    if (meta_role(meta) == JR_ROLE_LEADER) { L = r; ++nlead; }
-    else if (meta_role(meta) != JR_ROLE_FOLLOWER) return false;
-    if (meta_nq(meta)) return false;                                          // queued client requests
-  }
-  if (nlead != 1) return false;
-  s.L = L;
-  s.F0 = L == 0 ? 1u : 0u;
-  const uint4 l0 = d.p0[s.rg(L)];
-  s.term = (uint64_t)l0.x | ((uint64_t)l0.y << 32);
-  s.tbase = d.tb[s.g];
-  uint4 pl = p2[0], pf = p2[0];             // the leader's and the first follower's P2 (static selects: no local array)
-  const uint32_t f0i = L == 0 ? 1u : 0u;
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    if ((uint32_t)r == L) pl = p2[r];
-    if ((uint32_t)r == f0i) pf = p2[r];
-  }
-  s.head = pl.x; s.commit = pl.y; s.idgen = pl.z;
-  s.ckey = meta_ckey(pl.w);
-  s.maxkey = d.mk[s.rg(L)];
-  if (!(s.idgen > s.head)) return false;                                      // the next append would assert (chain.rs:163)
-  const uint4 l3 = d.p3[s.rg(L)];
-  s.hbtime = (uint64_t)l3.x | ((uint64_t)l3.y << 32);
-  // followers: identical
-  const uint32_t f0 = s.F0;
-  s.fhead = pf.x; s.fcommit = pf.y; s.fckey = meta_ckey(pf.w);
-  s.fmaxkey = d.mk[s.rg(f0)];
-  const uint64_t hbgap = ((uint64_t)d.hb / p.dt + 1) * p.dt;                 // ticks between two heartbeats, in ms
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    if ((uint32_t)r == L) continue;
-    const uint4 a = d.p0[s.rg(r)];
-    if (((uint64_t)a.x | ((uint64_t)a.y << 32)) != s.term || a.z != L + 1 || a.w != L + 1) return false;
-    if (p2[r].x != s.fhead || p2[r].y != s.fcommit || meta_ckey(p2[r].w) != s.fckey) return false;
-    if (d.mk[s.rg(r)] != s.fmaxkey) return false;
-  }
-  if ((uint64_t)d.emin <= hbgap || s.hbtime > p.now) return false;   // between two heartbeats no timer (>= emin) can fire
-  // the leader's view of the followers: one progress entry value for all of them
-  uint32_t ph[R];
-#pragma unroll
-  for (int q = 0; q < (R + 3) / 4; ++q) {
-    const uint4 v = d.pr[(size_t)q * s.plane + s.rg(L)];
-    if (q * 4 + 0 < R) ph[q * 4 + 0] = v.x;
-    if (q * 4 + 1 < R) ph[q * 4 + 1] = v.y;
-    if (q * 4 + 2 < R) ph[q * 4 + 2] = v.z;
-    if (q * 4 + 3 < R) ph[q * 4 + 3] = v.w;
-  }
-  const uint32_t prmask = meta_prmask(pl.w);
-  s.ph_self = 0; s.ph_f = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    if ((uint32_t)r == L) s.ph_self = ph[r];
-    if ((uint32_t)r == f0) s.ph_f = ph[r];
-  }
-  s.mode_self = (prmask >> L) & 1u;
-  s.mode_f = (prmask >> f0) & 1u;
-#pragma unroll
-  for (int r = 0; r < R; ++r)
-    if ((uint32_t)r != L && (ph[r] != s.ph_f || ((prmask >> r) & 1u) != s.mode_f)) return false;
-  // Everything the launch reads of a follower's table lies in [flo, fmaxkey] (or is written by the launch itself):
-  // the commit a heartbeat names (>= commit), the apply range (from fcommit), the parents of the blocks behind ph_f.
-  // Those rows must be identical in every follower, because the lowest follower's table stands for all of them; a read
-  // below flo that is not below the floor aborts the lane (fetch_f).  At most SYM_WINDOW ids, else step_kernel's business.
-  constexpr uint32_t SYM_WINDOW = 16;
-  const uint32_t top = min(s.maxkey, s.fmaxkey);
-  const uint32_t lo_min = max(top > SYM_WINDOW - 1u ? top - (SYM_WINDOW - 1u) : 0u, s.tbase);   // (below the floor nobody holds anything)
-  if (top < s.tbase || s.ph_f < lo_min || s.fcommit < lo_min || s.commit < lo_min || s.fhead < lo_min || s.fmaxkey > s.maxkey) return false;
-  const uint32_t lo = min(min(s.ph_f, s.fcommit), min(s.commit, s.fhead));
-  s.flo = lo;
-  const uint64_t grow = (uint64_t)p.n_ticks * (1u + p.n_synth) + 2u;
-  if ((uint64_t)s.maxkey + grow >= (uint64_t)s.tbase + d.cap || (uint64_t)s.maxkey + grow >= FS_NOTIFY_BIT) return false;
-  {  // batches of independent loads, no exit in between: one dependent load at a time would serialise ~100 latencies
-    constexpr uint32_t B = 4;
-    bool same = true;
-    for (uint32_t b0 = lo; b0 <= s.fmaxkey && same; b0 += B) {
-      uint32_t n0[B];
-      unsigned long long t0[B];
-#pragma unroll
-      for (uint32_t j = 0; j < B; ++j) {
-        const uint32_t b = min(b0 + j, s.fmaxkey);          // (the tail re-checks the last id: no divergent guards)
-        n0[j] = d.cnext[s.row(f0, b)];
-        t0[j] = d.ctok[s.row(f0, b)];
-      }
-#pragma unroll
-      for (int r = 0; r < R; ++r) {
-        if ((uint32_t)r == L || (uint32_t)r == f0) continue;
-#pragma unroll
-        for (uint32_t j = 0; j < B; ++j) {
-          const uint32_t b = min(b0 + j, s.fmaxkey);
-          const uint32_t n = d.cnext[s.row(r, b)];
-          const unsigned long long t = d.ctok[s.row(r, b)];
-          same = same && n == n0[j] && (n0[j] == ABSENT || t == t0[j]);
-        }
-      }
-    }
-    if (!same) return false;
-  }
-  // mail in flight (the previous tick's outboxes), delivered only with PH_DRAIN
-  m = SymMail{};
-  if (p.phases & PH_DRAIN) {
-  {  // leader: [Heartbeat to Peers] then one AppendEntries per peer, ascending, all carrying the same run
-    const uint32_t cnt = d.oc[prv][s.rg(L)];
-    uint32_t u = 0;
-    auto unit = [&](uint32_t k) { return d.ob[prv][((size_t)k * R + L) * d.Gp + s.g]; };
-    if (cnt > (uint32_t)(1 + JR_MAX_AE_BLOCKS + R)) return false;
-    if (u < cnt) {
-      const uint4 h = unit(u);
-      if ((h.x & 15u) == JR_CMD_HEARTBEAT) {
-        if ((h.x >> 16) != TO_PEERS || ((uint64_t)h.y | ((uint64_t)h.z << 32)) != s.term) return false;
-        m.hb = 1; m.hb_commit = h.w;
-        ++u;
-      }
-    }
-    if (u < cnt) {
-      uint32_t first = 0;
-      for (int r = 0; r < R; ++r) {
-        if ((uint32_t)r == L) continue;
-        if (u >= cnt) return false;
-        const uint4 h = unit(u);
-        if ((h.x & 15u) != JR_CMD_APPEND_ENTRIES || (h.x >> 16) != (uint32_t)r + 1u ||
-            ((uint64_t)h.y | ((uint64_t)h.z << 32)) != s.term) return false;
-        const uint32_t nb = (h.x >> 8) & 255u, ref = (h.x >> 4) & 1u;
-        if (!m.ae) {                                        // the first peer carries the run inline
-          if (ref || nb > JR_MAX_AE_BLOCKS || h.w != u + 1 || u + 1 + nb > cnt) return false;
-          m.ae = 1; m.ae_nb = nb; first = u + 1;
-          for (uint32_t k = 0; k < nb; ++k) {
-            const uint4 bu = unit(first + k);
-            uint32_t nx; uint64_t tk;
-            s.fetch(L, bu.x, nx, tk);                       // the sim re-reads the block from the leader's table: must be what was sent
-            if (nx != bu.y || tk != ((uint64_t)bu.z | ((uint64_t)bu.w << 32))) return false;
-            m.set_id(k, bu.x);
-          }
-          u += 1 + nb;
-        } else {                                            // the others point at it
-          if (!ref || nb != m.ae_nb || h.w != first) return false;
-          ++u;
-        }
-      }
-    }
-    if (u != cnt) return false;
-  }
-  {  // followers: [HeartbeatResponse][AppendResponse] to the leader, the same from each
-    const uint32_t cnt = d.oc[prv][s.rg(f0)];
-    if (cnt > 2) return false;
-    uint4 want[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-    for (uint32_t u = 0; u < cnt; ++u) want[u] = d.ob[prv][((size_t)u * R + f0) * d.Gp + s.g];
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-      if ((uint32_t)r == L || (uint32_t)r == f0) continue;
-      if (d.oc[prv][s.rg(r)] != cnt) return false;
-      for (uint32_t u = 0; u < cnt; ++u) {
-        const uint4 v = d.ob[prv][((size_t)u * R + r) * d.Gp + s.g];
-        if (v.x != want[u].x || v.y != want[u].y || v.z != want[u].z || v.w != want[u].w) return false;
-      }
-    }
-    uint32_t u = 0;
-    if (u < cnt && (want[u].x & 15u) == JR_CMD_HEARTBEAT_RESPONSE) {
-      if ((want[u].x >> 16) != L + 1) return false;
-      m.hbr = 1; m.hbr_has = (want[u].x >> 4) & 1u; m.hbr_commit = want[u].w;
-      ++u;
-    }
-    if (u < cnt && (want[u].x & 15u) == JR_CMD_APPEND_RESPONSE) {
-      if ((want[u].x >> 16) != L + 1 || ((uint64_t)want[u].y | ((uint64_t)want[u].z << 32)) != s.term) return false;
-      m.ar = 1; m.ar_head = want[u].w;
-      ++u;
-    }
-    if (u != cnt) return false;
-  }
-  }
-  // Election timers (mod.rs:352-357): no follower may time out before the first heartbeat of this launch reaches it.
-  // The leader heartbeats at the first tick with now - heartbeat_time > heartbeat_ms (leader.rs:78-84,237-240); the
-  // follower takes it one tick later, before its own Tick.  (Afterwards the static bound above holds.)
-  uint64_t t_arr = 0;
-  if (!m.hb) {
-    const uint64_t due = s.hbtime + (uint64_t)d.hb + 1;                     // smallest `now` that heartbeats
-    t_arr = (due > p.now ? (due - p.now + p.dt - 1) / p.dt : 0) + 1;
-  }
-  const uint64_t checked = t_arr < p.n_ticks ? t_arr : p.n_ticks;           // ticks whose Tick runs on the old timer
-  if (checked) {
-    const uint64_t t_last = p.now + (checked - 1) * p.dt;
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-      if ((uint32_t)r == L) continue;
-      const uint4 b = d.p1[s.rg(r)];
-      const uint64_t etime = (uint64_t)b.x | ((uint64_t)b.y << 32);
-      if (t_last >= etime && t_last - etime > (uint64_t)b.z) return false;
-    }
-  }
-  return true;
-}
-
 // ---- entry record ------------------------------------------------------------------------------------------------------
-// sym_check_kernel runs sym_enter for every group, one thread each, right before the fold kernel, and leaves its verdict
-// and everything the fold takes from the state planes in the entry record: [word][group] planes of 32-bit words (Gp
-// groups per plane), so that every warp's loads and stores are coalesced.  The fold kernels load the words of their
-// side in one round instead of walking sym_enter's chain of dependent loads with a quarter of the warps in flight.
+// sym_check_kernel (below) checks every group right before the fold kernel and leaves its verdict and everything the
+// fold takes from the state planes in the entry record: [word][group] planes of 32-bit words (Gp groups per plane), so
+// that every warp's loads and stores are coalesced.  The fold kernels load the words of their side in one round instead
+// of walking the entry checks' dependent loads with a quarter of the warps in flight.
 // Only sym_leave_* writes these planes of a folded group between the two kernels, so the words carried to the exit are
 // the ones it would read there.  Transient: rewritten by every pre-pass, not part of a checkpoint.
 //   SR_FLAGS      ok | L << 1 | ckey << 4 | fckey << 5 | mode_self << 6 | mode_f << 7 | mail in flight: hb << 8 | ae << 9 |
@@ -784,56 +578,290 @@ __host__ __device__ constexpr uint32_t sr_draws(uint32_t R) { return SR_P2W + (R
 __host__ __device__ constexpr uint32_t sr_idgen(uint32_t R) { return sr_draws(R) + R - 1; }
 __host__ __device__ constexpr uint32_t sym_record_words(uint32_t R) { return sr_idgen(R) + R - 1; }
 
-// One thread per group, 128-thread CTAs.  The checks are chains of dependent loads, so what makes them go faster is the
-// number of chains in flight -- but sym_enter wants ~126 registers, and spills cost more than warps gain: 5 CTAs per SM
-// (96 registers, no spills, 20 warps) ran the pre-pass in 45 us on the H100 at the headline shape, 8 CTAs (64
-// registers, 100 B of spill stores) in 49 us, 12 CTAs (40 registers, 492 B) in 55 us.  (A/B builds override it.)
-#ifndef JR_SYM_CHECK_MINCTAS
-#define JR_SYM_CHECK_MINCTAS 5
-#endif
-constexpr uint32_t SYM_CHECK_THREADS = 128;
+// ---- entry checks: is the group symmetric, is its mail canonical? ------------------------------------------------------
+// sym_check_kernel: one CTA per 32 consecutive groups and R warps, warp r = replica r of those groups (lane = group), so
+// that every load of a state plane, mailbox unit or table row is one coalesced 32-wide access and the loads of a round
+// are independent of each other.  Three rounds of loads, two barriers:
+//   1. every warp: its replica's P0..P2, max key, FSM counters, outbox count and first two outbox units, the floor; a
+//      warp whose replica is a leader also its P3 and progress entries.  Each posts what the checks need of its replica
+//      (SC_*, below) in shared memory.  Barrier: every lane now knows L, F0 and their words.
+//   2. follower warps compare their state, their rows [flo, fmaxkey] and their outbox with F0's and check their election
+//      timer; the leader's warp checks its own state and parses its outbox: the Heartbeat, the AppendEntries run and the
+//      headers that point at it ...
+//   3. ... and re-reads the run's <= 5 blocks from its table.
+// Each warp stages the record words of its side and posts a verdict word (no shared atomics, shuffles or votes: the host
+// build of the device code runs a CTA's threads as OS threads); after the second barrier the warps store the record word
+// by word, each store 32 consecutive groups.  Which check rejects a group first does not matter: the verdict and the
+// record are all that leaves the kernel, and every load stays inside its plane whatever the group holds.
+constexpr uint32_t SYM_WINDOW = 16;        // most follower rows compared: more, and the group is step_kernel's business
+enum : uint32_t {                          // words each warp posts for its replica, [slot][replica][lane]
+  SC_META = 0, SC_HEAD, SC_COMMIT, SC_IDGEN, SC_MK, SC_TERM, SC_TERM_HI,   // P2, max key, P0 .x .y
+  SC_VOTE,                                 // P0 .z (leader_id) if it equals P0 .w (voted_for), else 0
+  SC_FC, SC_FC_HI, SC_OC, SC_U0, SC_U1 = SC_U0 + 4,                        // FSM counters, outbox count, units 0 and 1
+  SC_PH_SELF = SC_U1 + 4, SC_PH_F, SC_HBTIME, SC_HBTIME_HI,               // a leader's (else 0)
+  SC_VERDICT,                              // after round 2: SC_FAIL | SC_NOSHARE | this replica's bits of SR_FLAGS
+  SC_SLOTS
+};
+constexpr uint32_t SC_FAIL = 1u, SC_NOSHARE = 1u << 31;   // (bit 0 of SR_FLAGS is `ok`; bits 17+ are unused there)
+// after the posts: the record staged [word][lane], then the leader's AppendEntries blocks {next, token} [3 * block][lane]
+__host__ __device__ constexpr uint32_t sym_check_smem_words(uint32_t R) {
+  return (SC_SLOTS * R + sym_record_words(R) + 3 * JR_MAX_AE_BLOCKS) * 32u;
+}
+// CTAs per SM the register allocation must allow: about 40 warps for every R, at 48 registers (52 at R = 6, 7) and no
+// spills.  (With 40 registers for 48 warps, every R from 4 up spills.)
+__host__ __device__ constexpr uint32_t sym_check_ctas(uint32_t R) { return 40u / R; }
+
 template <int R>
-__global__ void __launch_bounds__(SYM_CHECK_THREADS, JR_SYM_CHECK_MINCTAS) sym_check_kernel(const Dev d, const StepParams p, uint32_t* rec) {
-  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= d.Gp) return;
-  const size_t n = d.Gp;
-  uint32_t* w = rec + g;
-  SymGroup<R, true> s(d, g);
-  SymMail m;
-  if (!sym_enter(s, m, p, 1 - p.cur)) { w[SR_FLAGS * n] = 0u; return; }
-  const uint32_t L = s.L;
+__global__ void __launch_bounds__(32 * R, sym_check_ctas(R)) sym_check_kernel(const Dev d, const StepParams p, uint32_t* rec) {
+  JR_DYN_SMEM(uint32_t, sm);
+  const uint32_t r = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  const uint32_t g = blockIdx.x * 32u + lane;              // (Gp is a multiple of 32)
+  const size_t n = d.Gp, plane = (size_t)R * d.Gp, i = (size_t)r * d.Gp + g;
+  // Between the barriers a replica's words are read back from shared memory when a check needs them, not kept in registers.
+  auto post = [&](uint32_t slot, uint32_t q) -> uint32_t& { return sm[(slot * R + q) * 32u + lane]; };
+  auto post64 = [&](uint32_t slot, uint32_t q) { return (uint64_t)post(slot, q) | ((uint64_t)post(slot + 1, q) << 32); };
+  auto posted_unit = [&](uint32_t slot, uint32_t q) {
+    return make_uint4(post(slot, q), post(slot + 1, q), post(slot + 2, q), post(slot + 3, q));
+  };
+  uint32_t* stage = sm + SC_SLOTS * R * 32u + lane;       // the record, [word][lane]
+  auto put = [&](uint32_t word, uint32_t v) { stage[word * 32u] = v; };
+  uint32_t* blk = stage + sym_record_words(R) * 32u;
+  const int prv = 1 - p.cur;
   const bool cap = (d.flags & JR_F_CAPTURE_FSM) != 0;
-  bool share = cap;                                          // the followers' Instruction FIFOs are all empty
-  uint32_t hw[(R + 1) / 2];
-#pragma unroll
-  for (int k = 0; k < (R + 1) / 2; ++k) hw[k] = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    const uint4 c = d.p2[s.rg(r)];
-    hw[r / 2] |= ((c.w >> 16) & ~(1u << 12)) << (16 * (r & 1));
-    if ((uint32_t)r == L) continue;
-    const uint32_t k = (uint32_t)r - ((uint32_t)r > L ? 1u : 0u);
-    const uint2 fc = d.fc[s.rg(r)];
-    if (fc.x | fc.y) share = false;
-    w[(sr_draws(R) + k) * n] = d.p1[s.rg(r)].w;
-    w[(sr_idgen(R) + k) * n] = c.z;
+  auto unit = [&](uint32_t k) { return d.ob[prv][(size_t)k * plane + i]; };   // this replica's outbox unit k
+
+  // ---- round 1 ----
+  uint4 p0 = make_uint4(0u, 0u, 0u, 0u), p1 = p0, p2 = p0, u0 = p0, u1 = p0, p3 = p0;
+  uint2 fc = make_uint2(0u, 0u);
+  uint32_t mk = 0, tbase = 0, cnt = 0;
+  const bool in = g < d.G;
+  if (in) {
+    p0 = d.p0[i]; p1 = d.p1[i]; p2 = d.p2[i]; mk = d.mk[i]; fc = d.fc[i]; tbase = d.tb[g];
+    if (p.phases & PH_DRAIN) cnt = d.oc[prv][i];           // mail in flight (the previous tick's outboxes): PH_DRAIN only
   }
-  const uint2 fcl = cap ? d.fc[s.rg(L)] : make_uint2(0u, 0u);
-  w[SR_FLAGS * n] = 1u | (L << 1) | (s.ckey << 4) | (s.fckey << 5) | (s.mode_self << 6) | (s.mode_f << 7) | (m.hb << 8) |
-                    (m.ae << 9) | (m.ae_nb << 10) | (m.hbr << 13) | (m.hbr_has << 14) | (m.ar << 15) | ((share ? 1u : 0u) << 16);
-  w[SR_TBASE * n] = s.tbase;
-  w[SR_HEAD * n] = s.head; w[SR_COMMIT * n] = s.commit; w[SR_IDGEN * n] = s.idgen; w[SR_MAXKEY * n] = s.maxkey;
-  w[SR_PH_SELF * n] = s.ph_self; w[SR_PH_F * n] = s.ph_f;
-  w[SR_HBTIME * n] = (uint32_t)s.hbtime; w[(SR_HBTIME + 1) * n] = (uint32_t)(s.hbtime >> 32);
-  w[SR_HB_COMMIT * n] = m.hb_commit;
+  if (cnt > 0) u0 = unit(0);
+  if (cnt > 1) u1 = unit(1);
+  const uint32_t meta = p2.w;
+  const bool lead = meta_role(meta) == JR_ROLE_LEADER;
+  // roles: one live leader, R-1 live followers of that leader, no queued client requests
+  uint32_t v = !in || !meta_live(meta) || (!lead && meta_role(meta) != JR_ROLE_FOLLOWER) || meta_nq(meta) ? SC_FAIL : 0u;
+  uint32_t ph_self = 0, ph_f = 0;
+  if (lead) {
+    // the leader's view of the followers: one progress entry value and mode for all of them
+    const uint32_t f0 = r == 0 ? 1u : 0u;
+    p3 = d.p3[i];
+    uint32_t ph[R];
 #pragma unroll
-  for (uint32_t k = 0; k < JR_MAX_AE_BLOCKS; ++k) w[(SR_AE_ID + k) * n] = m.ae_id[k];
-  w[SR_FC_L * n] = fcl.x; w[(SR_FC_L + 1) * n] = fcl.y;
-  w[SR_FHEAD * n] = s.fhead; w[SR_FCOMMIT * n] = s.fcommit; w[SR_FMAXKEY * n] = s.fmaxkey; w[SR_FLO * n] = s.flo;
-  w[SR_HBR_COMMIT * n] = m.hbr_commit; w[SR_AR_HEAD * n] = m.ar_head;
-  w[SR_TERM * n] = (uint32_t)s.term; w[(SR_TERM + 1) * n] = (uint32_t)(s.term >> 32);
+    for (int q = 0; q < (R + 3) / 4; ++q) {
+      const uint4 e = d.pr[(size_t)q * plane + i];
+      if (q * 4 + 0 < R) ph[q * 4 + 0] = e.x;
+      if (q * 4 + 1 < R) ph[q * 4 + 1] = e.y;
+      if (q * 4 + 2 < R) ph[q * 4 + 2] = e.z;
+      if (q * 4 + 3 < R) ph[q * 4 + 3] = e.w;
+    }
+    const uint32_t prmask = meta_prmask(meta), mode_f = (prmask >> f0) & 1u;
 #pragma unroll
-  for (int k = 0; k < (R + 1) / 2; ++k) w[(SR_P2W + k) * n] = hw[k];
+    for (int q = 0; q < R; ++q) {                          // (static selects: no local array)
+      if ((uint32_t)q == r) ph_self = ph[q];
+      if ((uint32_t)q == f0) ph_f = ph[q];
+    }
+#pragma unroll
+    for (int q = 0; q < R; ++q)
+      if ((uint32_t)q != r && (ph[q] != ph_f || ((prmask >> q) & 1u) != mode_f)) v |= SC_FAIL;
+    v |= (r << 1) | (meta_ckey(meta) << 4) | (((prmask >> r) & 1u) << 6) | (mode_f << 7);
+  }
+  post(SC_META, r) = meta; post(SC_HEAD, r) = p2.x; post(SC_COMMIT, r) = p2.y; post(SC_IDGEN, r) = p2.z; post(SC_MK, r) = mk;
+  post(SC_TERM, r) = p0.x; post(SC_TERM_HI, r) = p0.y; post(SC_VOTE, r) = p0.z == p0.w ? p0.z : 0u;
+  post(SC_FC, r) = fc.x; post(SC_FC_HI, r) = fc.y; post(SC_OC, r) = cnt;
+  post(SC_U0, r) = u0.x; post(SC_U0 + 1, r) = u0.y; post(SC_U0 + 2, r) = u0.z; post(SC_U0 + 3, r) = u0.w;
+  post(SC_U1, r) = u1.x; post(SC_U1 + 1, r) = u1.y; post(SC_U1 + 2, r) = u1.z; post(SC_U1 + 3, r) = u1.w;
+  post(SC_PH_SELF, r) = ph_self; post(SC_PH_F, r) = ph_f; post(SC_HBTIME, r) = p3.x; post(SC_HBTIME_HI, r) = p3.y;
+  __syncthreads();
+
+  uint32_t L = 0, nlead = 0;
+#pragma unroll
+  for (int q = 0; q < R; ++q)
+    if (meta_role(post(SC_META, q)) == JR_ROLE_LEADER) { L = q; ++nlead; }
+  const uint32_t F0 = L == 0 ? 1u : 0u;                    // lowest follower: its block table stands for every follower's
+  // Everything the launch reads of a follower's table lies in [flo, fmaxkey] (or is written by the launch itself): the
+  // commit a heartbeat names (>= commit), the apply range (from fcommit), the parents of the blocks behind ph_f.  Those
+  // rows must be identical in every follower, because the lowest follower's table stands for all of them; a read below
+  // flo that is not below the floor aborts the lane (fetch_f).  At most SYM_WINDOW ids.  And the launch's appends must
+  // stay in the window and below 2^31.  true: all of that holds; lo = flo.
+  auto window = [&](uint32_t& lo) {
+    const uint32_t maxkey = post(SC_MK, L), commit = post(SC_COMMIT, L), phf = post(SC_PH_F, L);
+    const uint32_t fhead = post(SC_HEAD, F0), fcommit = post(SC_COMMIT, F0), fmaxkey = post(SC_MK, F0);
+    const uint32_t top = min(maxkey, fmaxkey);
+    const uint32_t lo_min = max(top > SYM_WINDOW - 1u ? top - (SYM_WINDOW - 1u) : 0u, tbase);   // (below the floor nobody holds anything)
+    lo = min(min(phf, fcommit), min(commit, fhead));
+    const uint64_t grow = (uint64_t)p.n_ticks * (1u + p.n_synth) + 2u;
+    return !(top < tbase || phf < lo_min || fcommit < lo_min || commit < lo_min || fhead < lo_min || fmaxkey > maxkey) &&
+           (uint64_t)maxkey + grow < (uint64_t)tbase + d.cap && (uint64_t)maxkey + grow < FS_NOTIFY_BIT;
+  };
+
+  // ---- rounds 2 and 3 ----
+  if (r == L) {
+    const uint64_t term = post64(SC_TERM, L), hbtime = post64(SC_HBTIME, L);
+    const uint64_t hbgap = ((uint64_t)d.hb / p.dt + 1) * p.dt;   // ticks between two heartbeats, in ms
+    if ((uint64_t)d.emin <= hbgap || hbtime > p.now) v |= SC_FAIL;   // between two heartbeats no timer (>= emin) can fire
+    if (!(post(SC_IDGEN, L) > post(SC_HEAD, L))) v |= SC_FAIL;     // the next append would assert (chain.rs:163)
+    uint32_t lo;
+    if (!window(lo)) v |= SC_FAIL;
+    // leader: [Heartbeat to Peers] then one AppendEntries per peer, ascending, all carrying the same run: the first
+    // peer's inline, the others pointing at it
+    SymMail m{};
+    const uint32_t cnt = post(SC_OC, L);
+    if (cnt > (uint32_t)(1 + JR_MAX_AE_BLOCKS + R)) v |= SC_FAIL;
+    else {
+      uint32_t u = 0;
+      const uint4 h0 = posted_unit(SC_U0, L);
+      if (u < cnt && (h0.x & 15u) == JR_CMD_HEARTBEAT) {
+        if ((h0.x >> 16) != TO_PEERS || ((uint64_t)h0.y | ((uint64_t)h0.z << 32)) != term) v |= SC_FAIL;
+        m.hb = 1; m.hb_commit = h0.w;
+        ++u;
+      }
+      if (u < cnt) {
+        const uint4 h = u ? posted_unit(SC_U1, L) : h0;
+        const uint32_t nb = (h.x >> 8) & 255u, first = u + 1;
+        // every other peer's header follows the run, so the count is first + nb + R - 2
+        if ((h.x & 15u) != JR_CMD_APPEND_ENTRIES || (h.x >> 16) != F0 + 1u || ((uint64_t)h.y | ((uint64_t)h.z << 32)) != term ||
+            ((h.x >> 4) & 1u) || nb > JR_MAX_AE_BLOCKS || h.w != first || first + nb + R - 2 != cnt) {
+          v |= SC_FAIL;
+        } else {
+          m.ae = 1; m.ae_nb = nb;
+#pragma unroll
+          for (uint32_t k = 0; k < JR_MAX_AE_BLOCKS; ++k)
+            if (k < nb) {
+              const uint4 b = unit(first + k);
+              m.ae_id[k] = b.x;
+              blk[(3 * k) * 32u] = b.y; blk[(3 * k + 1) * 32u] = b.z; blk[(3 * k + 2) * 32u] = b.w;
+            }
+#pragma unroll
+          for (uint32_t j = 1; j + 1 < (uint32_t)R; ++j) {
+            const uint32_t peer = j + (j >= L ? 1u : 0u);
+            const uint4 o = unit(first + nb + j - 1);
+            if ((o.x & 15u) != JR_CMD_APPEND_ENTRIES || (o.x >> 16) != peer + 1u || ((uint64_t)o.y | ((uint64_t)o.z << 32)) != term ||
+                !((o.x >> 4) & 1u) || ((o.x >> 8) & 255u) != nb || o.w != first) v |= SC_FAIL;
+          }
+          // the sim re-reads each block from the leader's table: it must be what was sent
+#pragma unroll
+          for (uint32_t k = 0; k < JR_MAX_AE_BLOCKS; ++k)
+            if (k < nb) {
+              const uint32_t bid = m.ae_id[k];
+              uint32_t nx = ABSENT;
+              unsigned long long tk = 0;
+              if (bid - tbase < d.cap) {
+                const size_t row = table_row(d, plane, bid, i);
+                nx = d.cnext[row];
+                tk = d.ctok[row];
+              }
+              if (nx != blk[(3 * k) * 32u] ||
+                  tk != ((unsigned long long)blk[(3 * k + 1) * 32u] | ((unsigned long long)blk[(3 * k + 2) * 32u] << 32))) v |= SC_FAIL;
+            }
+        }
+      }
+    }
+    v |= (m.hb << 8) | (m.ae << 9) | (m.ae_nb << 10);
+    put(SR_HEAD, post(SC_HEAD, L)); put(SR_COMMIT, post(SC_COMMIT, L)); put(SR_IDGEN, post(SC_IDGEN, L));
+    put(SR_MAXKEY, post(SC_MK, L)); put(SR_PH_SELF, post(SC_PH_SELF, L)); put(SR_PH_F, post(SC_PH_F, L));
+    put(SR_HBTIME, (uint32_t)hbtime); put(SR_HBTIME + 1, (uint32_t)(hbtime >> 32));
+    put(SR_HB_COMMIT, m.hb_commit);
+#pragma unroll
+    for (uint32_t k = 0; k < JR_MAX_AE_BLOCKS; ++k) put(SR_AE_ID + k, m.ae_id[k]);
+    put(SR_FC_L, cap ? post(SC_FC, L) : 0u); put(SR_FC_L + 1, cap ? post(SC_FC_HI, L) : 0u);
+    put(SR_TERM, (uint32_t)term); put(SR_TERM + 1, (uint32_t)(term >> 32));
+  } else {
+    // followers: voted for the leader, identical to F0
+    if (post64(SC_TERM, r) != post64(SC_TERM, L) || post(SC_VOTE, r) != L + 1 || post(SC_HEAD, r) != post(SC_HEAD, F0) ||
+        post(SC_COMMIT, r) != post(SC_COMMIT, F0) || post(SC_MK, r) != post(SC_MK, F0) ||
+        meta_ckey(post(SC_META, r)) != meta_ckey(post(SC_META, F0))) v |= SC_FAIL;
+    // Election timers (mod.rs:352-357): no follower may time out before the first heartbeat of this launch reaches it.
+    // The leader heartbeats at the first tick with now - heartbeat_time > heartbeat_ms (leader.rs:78-84,237-240); the
+    // follower takes it one tick later, before its own Tick.  (Afterwards the leader's bound above holds.)
+    uint64_t t_arr = 0;
+    if (!(post(SC_OC, L) > 0 && (post(SC_U0, L) & 15u) == JR_CMD_HEARTBEAT)) {   // no Heartbeat in flight
+      const uint64_t due = post64(SC_HBTIME, L) + (uint64_t)d.hb + 1;          // smallest `now` that heartbeats
+      t_arr = (due > p.now ? (due - p.now + p.dt - 1) / p.dt : 0) + 1;
+    }
+    const uint64_t checked = t_arr < p.n_ticks ? t_arr : p.n_ticks;   // ticks whose Tick runs on the old timer
+    if (checked) {
+      const uint64_t t_last = p.now + (checked - 1) * p.dt;
+      const uint64_t etime = (uint64_t)p1.x | ((uint64_t)p1.y << 32);
+      if (t_last >= etime && t_last - etime > (uint64_t)p1.z) v |= SC_FAIL;
+    }
+    if (cap && (post(SC_FC, r) | post(SC_FC_HI, r))) v |= SC_NOSHARE;   // records pending: each follower gets its own
+    const uint32_t k = r - (r > L ? 1u : 0u);
+    put(sr_draws(R) + k, p1.w);
+    put(sr_idgen(R) + k, post(SC_IDGEN, r));
+    const uint32_t fcnt = post(SC_OC, F0);                 // F0's mail: [HeartbeatResponse][AppendResponse] to the leader
+    if (fcnt > 2) v |= SC_FAIL;
+    uint32_t lo;
+    const bool win = window(lo);
+    if (r != F0) {
+      // the same mail as F0
+      if (post(SC_OC, r) != fcnt) v |= SC_FAIL;
+#pragma unroll
+      for (uint32_t w = 0; w < 8; ++w)
+        if (w < 4 * fcnt && post(SC_U0 + w, r) != post(SC_U0 + w, F0)) v |= SC_FAIL;
+      // the same rows [flo, fmaxkey] as F0, in batches of independent loads
+      const uint32_t fmaxkey = post(SC_MK, F0);
+      const size_t i0 = (size_t)F0 * n + g;
+      constexpr uint32_t B = 2;
+      bool same = true;
+      if (win)
+        for (uint32_t b0 = lo; b0 <= fmaxkey && same; b0 += B) {
+          uint32_t n0[B], n1[B];
+          unsigned long long t0[B], t1[B];
+#pragma unroll
+          for (uint32_t j = 0; j < B; ++j) {
+            const uint32_t b = min(b0 + j, fmaxkey);        // (the tail re-checks the last id: no divergent guards)
+            n0[j] = d.cnext[table_row(d, plane, b, i0)]; t0[j] = d.ctok[table_row(d, plane, b, i0)];
+            n1[j] = d.cnext[table_row(d, plane, b, i)]; t1[j] = d.ctok[table_row(d, plane, b, i)];
+          }
+#pragma unroll
+          for (uint32_t j = 0; j < B; ++j) same = same && n1[j] == n0[j] && (n0[j] == ABSENT || t1[j] == t0[j]);
+        }
+      if (!same) v |= SC_FAIL;
+    } else {
+      SymMail m{};
+      const uint32_t cnt = fcnt;
+      const uint4 h0 = posted_unit(SC_U0, r);
+      uint32_t u = 0;
+      if (u < cnt && (h0.x & 15u) == JR_CMD_HEARTBEAT_RESPONSE) {
+        if ((h0.x >> 16) != L + 1) v |= SC_FAIL;
+        m.hbr = 1; m.hbr_has = (h0.x >> 4) & 1u; m.hbr_commit = h0.w;
+        ++u;
+      }
+      const uint4 a = u ? posted_unit(SC_U1, r) : h0;
+      if (u < cnt && (a.x & 15u) == JR_CMD_APPEND_RESPONSE) {
+        if ((a.x >> 16) != L + 1 || ((uint64_t)a.y | ((uint64_t)a.z << 32)) != post64(SC_TERM, L)) v |= SC_FAIL;
+        m.ar = 1; m.ar_head = a.w;
+        ++u;
+      }
+      if (u != cnt) v |= SC_FAIL;
+      v |= (meta_ckey(post(SC_META, r)) << 5) | (m.hbr << 13) | (m.hbr_has << 14) | (m.ar << 15);
+      put(SR_TBASE, tbase);
+      put(SR_FHEAD, post(SC_HEAD, r)); put(SR_FCOMMIT, post(SC_COMMIT, r)); put(SR_FMAXKEY, post(SC_MK, r)); put(SR_FLO, lo);
+      put(SR_HBR_COMMIT, m.hbr_commit); put(SR_AR_HEAD, m.ar_head);
+    }
+  }
+  if (!(r & 1u)) {   // the upper half of P2 .w with ckey cleared, replicas r and r + 1
+    const uint32_t hi = (uint32_t)r + 1 < (uint32_t)R ? ((post(SC_META, r + 1) >> 16) & ~(1u << 12)) << 16 : 0u;
+    put(SR_P2W + r / 2, ((post(SC_META, r) >> 16) & ~(1u << 12)) | hi);
+  }
+  post(SC_VERDICT, r) = v;
+  __syncthreads();
+
+  uint32_t all = 0;
+#pragma unroll
+  for (int q = 0; q < R; ++q) all |= post(SC_VERDICT, q);
+  const bool ok = !(all & SC_FAIL) && nlead == 1;
+  for (uint32_t k = r; k < sym_record_words(R); k += R) {
+    if (k == SR_FLAGS)
+      rec[g] = ok ? 1u | (all & 0xfffeu) | ((cap && !(all & SC_NOSHARE) ? 1u : 0u) << 16) : 0u;
+    else if (ok)
+      rec[k * n + g] = stage[k * 32u];
+  }
 }
 
 // The entry record of group s.g (< Gp), one round of loads: LEAD the leader's side (and fc = its FSM counters), FOLLOW
@@ -1099,7 +1127,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
           SymMail in{}, out{};
           in.hb = ma.x & 1u; in.ae = (ma.x >> 1) & 1u;
           in.hb_commit = ma.y; in.mk = ma.z;
-          if (ma.x & SYM2_IDS) {                           // tick 0: the blocks sym_enter found in the leader's outbox
+          if (ma.x & SYM2_IDS) {                           // tick 0: the blocks sym_check_kernel found in the leader's outbox
             const uint4 mb = mail[(2 * (1 - cur) + 1) * S];
             in.ae_nb = (ma.x >> 4) & 15u;
             in.ae_id[0] = ma.w; in.ae_id[1] = mb.x; in.ae_id[2] = mb.y; in.ae_id[3] = mb.z; in.ae_id[4] = mb.w;
