@@ -38,6 +38,8 @@
  *                         every node at once, chain.rs:119-123,198, plus the volatile State the reference loses)
  *   jr_truncate        <- no reference API (deviation D7)
  *   jr_group_export / jr_group_import <- no reference API: reassigning a group to another engine
+ *   jr_set_links / jr_get_links / jr_isolate_leaders <- no reference API: a tcp.rs connection that delivers nothing
+ *                         (deviation D8)
  *
  * One engine = G independent Raft groups x R replicas, all resident in one GPU's
  * HBM.  The reference is one group, one node per process; the group dimension is
@@ -72,6 +74,10 @@
  *       must then lie in [floor, floor + chain_capacity).  Removed keys read as absent, exactly as
  *       if sled had lost them (has() false, range() skips them).  An engine that never calls
  *       jr_truncate behaves as before (floor 0).
+ *   D8  peer-link cuts (JR_F_PEER_LINKS): mail over a cut link is DROPPED at delivery.  The reference
+ *       keeps it: while a TCP connect fails, the message stays in the sender's channel and goes out
+ *       once the connection is back (tcp.rs:110-135, connect_and_send).  Delayed delivery is not
+ *       modelled; the schedule already drops mail that is not delivered in the next step.
  *
  * All structs are plain data, little endian, naturally aligned.  No callbacks.
  * Buffers passed to jr_step are HOST memory owned by the caller.
@@ -162,8 +168,11 @@ enum {
   JR_F_STREAM_DIGEST = 1u << 3,          /* keep the running digests jr_stream_digest returns  */
   JR_F_NO_SYMMETRIC_FOLD = 1u << 4,      /* jr_run* never take the symmetric-group fast path (DESIGN.md section 3b); results are
                                           * identical either way -- the flag exists for A/B measurements and tests      */
-  JR_F_CLIENT_RESPONSES = 1u << 5        /* every drain also runs fsm::Driver's notification map on the device and returns the
+  JR_F_CLIENT_RESPONSES = 1u << 5,       /* every drain also runs fsm::Driver's notification map on the device and returns the
                                           * ClientResponses it produces (jr_fsm_responses).  Requires JR_F_CAPTURE_FSM */
+  JR_F_PEER_LINKS = 1u << 6              /* each group keeps a link matrix: jr_set_links / jr_get_links / jr_isolate_leaders
+                                          * cut and heal the connections between its replicas (D8).  Without the flag those
+                                          * calls return JR_E_INVAL and nothing is allocated */
 };
 
 /* ---- configuration (RaftConfig, src/raft/config.rs:14-41, batched) --------- */
@@ -694,6 +703,36 @@ jr_status jr_group_import(jr_engine* e, const uint32_t* slots, size_t n, const v
 
 /* Silence the current leader of every group g with hash(seed,g,salt) % 1000 < permille. */
 jr_status jr_kill_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64_t* n_killed);
+
+/*
+ * ---- peer links (JR_F_PEER_LINKS; deviation D8) --------------------------------------------------------------------
+ * Normative:
+ * Each group has a 64-bit link matrix.  Bit 8*(r-1) + (s-1) set: mail from node s to node r of this group is not
+ * delivered.  A cut is directional (a symmetric partition sets both bits).  Bits on the diagonal (r == s) and bits that
+ * name a node above n_replicas are refused.  A new engine, and every jr_engine_reset, starts fully connected (all zero).
+ *   What is dropped: at delivery (schedule item 1 of jr_step_args) receiver r skips every unit of a sender whose bit is
+ *   set in its row -- mail addressed to it and Peers broadcasts alike.  The mail is dropped, not delayed (D8).
+ *   What is not affected: emission (the stream digests, n_msgs and jr_step's out_msgs hold every Message emitted);
+ *   jr_step's inject[] entries (the host is the network for injected mail); proposals, Tick, jr_set_alive, restarts,
+ *   truncation, compaction and verification.  A cut-off replica is still alive, so it still holds jr_truncate's floor
+ *   down: with truncation, a long partition ends with the majority's leader faulting with
+ *   JR_FAULT_ENGINE_CHAIN_CAPACITY once its window is full, as in the reference's restatement.
+ *   When: the matrix is read at delivery.  A cut or heal set between two calls applies to every delivery after it, mail
+ *   already in flight included.  It never changes inside a jr_run* call.
+ *   Carried by jr_engine_save / jr_engine_restore and by group images (jr_group_import gives the slot the image's
+ *   matrix; jr_group_export leaves the source slot's as it was).  jr_state_digest does not include it.
+ * All three calls are synchronous on the engine stream and all or nothing: JR_E_INVAL leaves the engine untouched (also
+ * for an engine created without the flag).
+ */
+/* The matrix of groups[i] becomes cuts[i].  groups == NULL: n == n_groups and cuts is dense, one entry per group (all
+ * zeros heals everything).  JR_E_INVAL for a group out of range or named twice, or a refused bit. */
+jr_status jr_set_links(jr_engine* e, const uint32_t* groups, const uint64_t* cuts, size_t n);
+/* out[i] = the matrix of groups[i]; groups == NULL: n == n_groups, every group. */
+jr_status jr_get_links(jr_engine* e, const uint32_t* groups, size_t n, uint64_t* out);
+/* The partition counterpart of jr_kill_leaders: the same groups for the same salt and permille.  In each, every link to
+ * and from each live leader is cut (ORed into the matrix): the leader stays alive but reaches no one and hears no one.
+ * *n_isolated = the selected groups that had a live leader (also at n_replicas = 1, where there is no link to cut). */
+jr_status jr_isolate_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64_t* n_isolated);
 
 /* ---- leader announce ------------------------------------------------------- */
 /* Writes n_groups entries to DEVICE memory `dev_out` (for a collective) */

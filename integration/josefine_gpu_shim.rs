@@ -196,6 +196,13 @@ extern "C" {
     #[allow(dead_code)]
     fn jr_verify_groups(e: *mut c_void, groups: *const u32, n_groups: usize, report: *mut JrVerifyReport,
                         findings: *mut JrVerifyFinding, cap: usize, n_findings: *mut usize) -> c_int;
+    // peer-link cuts (JR_F_PEER_LINKS, deviation D8): bit 8*(r-1) + (s-1) of a group's matrix = mail s -> r is dropped
+    #[allow(dead_code)]
+    fn jr_set_links(e: *mut c_void, groups: *const u32, cuts: *const u64, n: usize) -> c_int;
+    #[allow(dead_code)]
+    fn jr_get_links(e: *mut c_void, groups: *const u32, n: usize, out: *mut u64) -> c_int;
+    #[allow(dead_code)]
+    fn jr_isolate_leaders(e: *mut c_void, salt: u64, permille: u32, n_isolated: *mut u64) -> c_int;
 }
 
 /// jr_verify_report: what one jr_verify_groups call checked, and its findings per kind.

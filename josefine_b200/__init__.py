@@ -7,7 +7,7 @@ raft.py the host-side mirror of the reference's Command / Apply interface.
 from . import abi  # noqa: F401
 from .fsm import BatchedDriver, ClientResponse  # noqa: F401
 from .raft import (Address, Command, RaftApi, RaftEngine, RaftError, ReplicaHandle,  # noqa: F401
-                   StepResult, expand_responses, fsm_tuple, load_engine_library, msg_tuple)
+                   StepResult, expand_responses, fsm_tuple, link_cut, load_engine_library, msg_tuple, partition)
 
 __all__ = ["abi", "BatchedDriver", "ClientResponse", "Address", "Command", "RaftApi", "RaftEngine", "RaftError", "ReplicaHandle",
-           "StepResult", "expand_responses", "fsm_tuple", "msg_tuple", "load_engine_library"]
+           "StepResult", "expand_responses", "fsm_tuple", "msg_tuple", "load_engine_library", "link_cut", "partition"]

@@ -52,6 +52,7 @@ F_CAPTURE_FSM = 1 << 2
 F_STREAM_DIGEST = 1 << 3
 F_NO_SYMMETRIC_FOLD = 1 << 4
 F_CLIENT_RESPONSES = 1 << 5
+F_PEER_LINKS = 1 << 6
 
 # step flags
 STEP_DELIVER = 1 << 0
@@ -216,6 +217,7 @@ ENGINE_SYMBOLS = [
     "jr_set_alive", "jr_kill_leaders", "jr_leader_table_device", "jr_leader_table", "jr_leader_table_async", "jr_leader_table_wait",
     "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_responses", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
     "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_verify_groups", "jr_group_export", "jr_group_import", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
+    "jr_set_links", "jr_get_links", "jr_isolate_leaders",
 ]
 
 

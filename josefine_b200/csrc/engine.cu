@@ -465,6 +465,45 @@ __global__ void kill_leaders_kernel(const Dev d, uint64_t base, uint32_t permill
   if (killed) atomicAdd(n_killed, (unsigned long long)killed);
 }
 
+// jr_isolate_leaders: kill_leaders_kernel's selection; each live leader of a picked group loses every link to and from it.
+__global__ void isolate_leaders_kernel(const Dev d, uint64_t base, uint32_t permille, unsigned long long* n_isolated) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool pick = g < d.G && mix64(base + d.goff + g) % 1000 < permille;
+  bool hit = false;   // the group has a live leader (at R = 1 it has no link to cut, and still counts)
+  if (pick) {
+    const unsigned long long row = (1ull << d.R) - 1ull;   // one row: every sender 1..R
+    unsigned long long col = 0, m = 0;                      // one column: every receiver 1..R
+    for (uint32_t r = 0; r < d.R; ++r) col |= 1ull << (8u * r);
+    for (uint32_t r = 0; r < d.R; ++r) {
+      const uint32_t meta = d.p2[(size_t)r * d.Gp + g].w;
+      if (meta_role(meta) == JR_ROLE_LEADER && meta_live(meta)) {
+        m |= (row << (8u * r)) | (col << r);
+        hit = true;
+      }
+    }
+    for (uint32_t r = 0; r < d.R; ++r) m &= ~(1ull << (9u * r));   // (the diagonal stays clear)
+    if (m) d.links[g] |= m;
+  }
+#ifdef JR_EMU
+  const uint32_t isolated = hit ? 1u : 0u;
+#else
+  // warp-aggregated count: one vote per lane, popcount of the ballot, one atomic per warp
+  const uint32_t votes = __ballot_sync(0xffffffffu, hit);
+  const uint32_t isolated = (threadIdx.x & 31u) == 0 ? (uint32_t)__popc(votes) : 0u;
+#endif
+  if (isolated) atomicAdd(n_isolated, (unsigned long long)isolated);
+}
+
+// jr_set_links / jr_get_links with a group list: in = {cuts[0 .. n), groups[0 .. n)}, host-validated.
+__global__ void links_scatter_kernel(const Dev d, const unsigned long long* cuts, const uint32_t* groups, uint32_t n) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) d.links[groups[k]] = cuts[k];
+}
+__global__ void links_gather_kernel(const Dev d, const uint32_t* groups, uint32_t n, unsigned long long* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) out[k] = d.links[groups[k]];
+}
+
 __global__ void set_alive_kernel(const Dev d, uint32_t g, uint32_t r, int alive) {
   const size_t i = (size_t)r * d.Gp + g;
   const uint32_t m = d.p2[i].w;
@@ -1627,6 +1666,7 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
   A(e->symdone, d.Gp);
   A(e->symblk, d.Gp / GROUPS_PER_CTA);
   A(e->symrec, (size_t)sym_record_words(d.R) * d.Gp);
+  if (d.flags & JR_F_PEER_LINKS) A(d.links, d.Gp);   // (padded groups too: step_kernel's lanes read their row)
   if (d.flags & JR_F_CAPTURE_FSM) {
     const size_t reps = (size_t)cfg->n_groups * cfg->n_replicas;   // default: 2 per replica, but never less than a small engine's whole FIFO space
     const size_t want = cfg->fsm_host_records ? cfg->fsm_host_records
@@ -1773,6 +1813,7 @@ jr_status jr_engine_reset(jr_engine* e) {
   if (e->rp.pnc)   // every fsm::Driver map empty, no restart pending
     CK(cudaMemsetAsync(e->rp.pnc, 0, ((plane + 3) / 4 + plane) * sizeof(uint4), e->stream));
   e->resp_b = -1;
+  if (d.links) CK(cudaMemsetAsync(d.links, 0, (size_t)d.Gp * sizeof(unsigned long long), e->stream));   // fully connected
   JR_LAUNCH(init_kernel, (unsigned)((plane + 255) / 256), 256, e->stream, d);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -3094,6 +3135,8 @@ std::vector<PlaneDesc> engine_planes(jr_engine* e) {
     v.push_back({e->rp.pnc, (plane + 3) / 4 * sizeof(uint4), Carry::WORDS, 1});
     v.push_back({e->rp.rm, plane * sizeof(uint4), Carry::WORDS, 4});
   }
+  if (d.links)   // the link matrices (JR_F_PEER_LINKS only, for the same reason)
+    v.push_back({d.links, (size_t)d.Gp * sizeof(unsigned long long), Carry::WORDS, 2, 1, true});
   return v;
 }
 
@@ -3404,6 +3447,90 @@ jr_status jr_kill_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64
   CK(cudaMemcpyAsync(&k, e->scratch, sizeof k, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   if (n_killed) *n_killed = k;
+  return JR_OK;
+}
+
+// ---- peer links (JR_F_PEER_LINKS) ------------------------------------------------------------------------------------
+// The bits a link matrix of an R-replica group may hold: 8*(r-1) + (s-1) for receivers and senders 1..R, r != s.
+static uint64_t links_valid_mask(uint32_t R) {
+  uint64_t m = 0;
+  for (uint32_t r = 0; r < R; ++r) m |= (((1ull << R) - 1ull) & ~(1ull << r)) << (8u * r);
+  return m;
+}
+
+// groups == NULL: n must be G (dense).  Otherwise every group in range and named once.  Checked on the host first.
+static jr_status links_check_groups(jr_engine* e, const uint32_t* groups, size_t n, const char* what) {
+  if (!e->d.links) { set_err("%s: engine created without JR_F_PEER_LINKS", what); return JR_E_INVAL; }
+  if (!groups) {
+    if (n != e->d.G) { set_err("%s: groups == NULL needs n == n_groups", what); return JR_E_INVAL; }
+    return JR_OK;
+  }
+  if (n > e->d.G) { set_err("%s: more groups than the engine holds", what); return JR_E_INVAL; }
+  std::vector<uint8_t> seen(e->d.G, 0);
+  for (size_t k = 0; k < n; ++k) {
+    if (groups[k] >= e->d.G || seen[groups[k]]) { set_err("%s: groups[%zu] out of range or named twice", what, k); return JR_E_INVAL; }
+    seen[groups[k]] = 1;
+  }
+  return JR_OK;
+}
+
+jr_status jr_set_links(jr_engine* e, const uint32_t* groups, const uint64_t* cuts, size_t n) {
+  if (!e || (n && !cuts)) return JR_E_INVAL;
+  jr_status st = links_check_groups(e, groups, n, "jr_set_links");
+  if (st != JR_OK) return st;
+  const uint64_t bad = ~links_valid_mask(e->d.R);
+  for (size_t k = 0; k < n; ++k)
+    if (cuts[k] & bad) { set_err("jr_set_links: cuts[%zu] has a bit on the diagonal or above n_replicas", k); return JR_E_INVAL; }
+  if (n == 0) return JR_OK;
+  CK(cudaSetDevice(e->cfg.device));
+  if (!groups) {
+    CK(cudaMemcpyAsync(e->d.links, cuts, n * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
+  } else {   // one copy: {cuts, groups}, then the scatter
+    std::vector<unsigned char> in(n * (sizeof(uint64_t) + sizeof(uint32_t)));
+    memcpy(in.data(), cuts, n * sizeof(uint64_t));
+    memcpy(in.data() + n * sizeof(uint64_t), groups, n * sizeof(uint32_t));
+    if ((st = many_reserve(e, in.size())) != JR_OK) return st;
+    CK(cudaMemcpyAsync(e->many_buf, in.data(), in.size(), cudaMemcpyHostToDevice, e->stream));
+    JR_LAUNCH(links_scatter_kernel, (unsigned)((n + 127) / 128), 128, e->stream, e->d, (const unsigned long long*)e->many_buf,
+              (const uint32_t*)((char*)e->many_buf + n * sizeof(uint64_t)), (uint32_t)n);
+    CK(cudaGetLastError());
+  }
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
+}
+
+jr_status jr_get_links(jr_engine* e, const uint32_t* groups, size_t n, uint64_t* out) {
+  if (!e || (n && !out)) return JR_E_INVAL;
+  jr_status st = links_check_groups(e, groups, n, "jr_get_links");
+  if (st != JR_OK) return st;
+  if (n == 0) return JR_OK;
+  CK(cudaSetDevice(e->cfg.device));
+  if (!groups) {
+    CK(cudaMemcpyAsync(out, e->d.links, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+  } else {   // the group list in, the gather, the matrices out
+    if ((st = many_reserve(e, n * (sizeof(uint64_t) + sizeof(uint32_t)))) != JR_OK) return st;
+    unsigned long long* dout = (unsigned long long*)e->many_buf;
+    uint32_t* dgroups = (uint32_t*)(dout + n);
+    CK(cudaMemcpyAsync(dgroups, groups, n * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    JR_LAUNCH(links_gather_kernel, (unsigned)((n + 127) / 128), 128, e->stream, e->d, (const uint32_t*)dgroups, (uint32_t)n, dout);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, dout, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+  }
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
+}
+
+jr_status jr_isolate_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64_t* n_isolated) {
+  if (!e) return JR_E_INVAL;
+  if (!e->d.links) { set_err("jr_isolate_leaders: engine created without JR_F_PEER_LINKS"); return JR_E_INVAL; }
+  CK(cudaSetDevice(e->cfg.device));
+  CK(cudaMemsetAsync(e->scratch, 0, sizeof(unsigned long long), e->stream));
+  JR_LAUNCH(isolate_leaders_kernel, (e->d.G + 127) / 128, 128, e->stream, e->d, mix64(e->d.seed ^ salt), permille, e->scratch);
+  CK(cudaGetLastError());
+  uint64_t k = 0;
+  CK(cudaMemcpyAsync(&k, e->scratch, sizeof k, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (n_isolated) *n_isolated = k;
   return JR_OK;
 }
 

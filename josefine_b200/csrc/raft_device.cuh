@@ -65,6 +65,7 @@ struct Dev {
   uint32_t* scatter;               // [0] set by a launch when some CTA has leaders on >= 2 replica indices;
                                    // [1] task ticket counter of the running step launch (both zeroed per launch)
   uint32_t* done;                  // [CTA-sized group block]: epoch + parts finished (split launches, see step_kernel)
+  unsigned long long* links;       // JR_F_PEER_LINKS, else null: [group] link matrix, bit 8*(r-1)+(s-1) = mail s -> r is cut
   unsigned long long* prof;        // JR_PROFILE builds: cycle counters [role 3][slot 16] x {cycles, count}
 #ifdef JR_SYM_ABORT_LOG
   uint32_t* sab;                   // [lane 2][group]: the fold's first abort site | tick << 8 (sym_fold.cuh, SA_*)
@@ -404,6 +405,7 @@ struct Replica {
   // (the stream digests and counts of JR_F_STREAM_DIGEST stay in d.dg / d.cn: a test feature must not cost the
   //  product kernel six registers)
   uint32_t mko[R];       // delivery index of this tick's outbox, one mask per receiver (see Local::mk_out)
+  uint32_t cut;          // senders (bit s = replica index s) whose mail this replica does not receive (JR_F_PEER_LINKS)
 
   __device__ __forceinline__ Replica(const Dev& dv, const Local& lv, uint32_t r_, uint32_t g_)
       : d(dv), L(lv), r(r_), g(g_), rg((size_t)r_ * dv.Gp + g_), plane((size_t)R * dv.Gp) {}
@@ -423,6 +425,7 @@ struct Replica {
     nq = meta_nq(m); dead = meta_dead(m); ckey = meta_ckey(m);
     maxkey = d.mk[rg];
     tbase = d.tb[g];
+    cut = d.links ? (uint32_t)(d.links[g] >> (8u * r)) & 255u : 0u;   // this replica's row; constant within a launch
     hbtime = 0;
 #pragma unroll
     for (int i = 0; i < (R < 3 ? 3 : R); ++i) ph[i] = 0;
@@ -1113,14 +1116,15 @@ struct Replica {
     uint32_t tail, tail_i;  // trailing schedule entries: see next_tail
   };
 
-  // Which senders have mail for me this tick: one shared-memory read per peer, up front.
+  // Which senders have mail for me this tick: one shared-memory read per peer, up front.  Every delivery path (leader
+  // fast drain, indexed, scan) starts from k.pend, so the senders whose links to me are cut are dropped here, once.
   __device__ __forceinline__ void plan_tick(Pos& k, const StepParams& p) const {
     k.pend = 0; k.s = 0; k.idx = 0; k.u = 0; k.cnt = 0; k.reps = 0; k.rep_at = 0;
     if (p.phases & PH_DRAIN) {
 #pragma unroll
       for (int s_ = 0; s_ < R; ++s_)
         if (d.use_index ? (uint32_t)L.mk_in[(r * R + s_) * 32 + L.lane] : L.cin[s_ * 32 + L.lane]) k.pend |= 1u << s_;
-      k.pend &= ~(1u << r);  // never my own mailbox
+      k.pend &= ~((1u << r) | cut);  // never my own mailbox, nor a cut link's
     }
     k.tail = 0;
   }

@@ -25,7 +25,8 @@
 //     exact unit layout step_kernel produces, and the Instruction streams leave through the same streaming encoder
 //     fsm_flush uses (fsm_enc_push), fed as the Instructions are produced.
 //   * Stream digests (JR_F_STREAM_DIGEST) need every Message in order, which this path never materialises: engines
-//     created with that flag, or with JR_F_SLED_COMMIT_KEY_STRICT / JR_F_NO_SYMMETRIC_FOLD, never take it.
+//     created with that flag, or with JR_F_SLED_COMMIT_KEY_STRICT / JR_F_NO_SYMMETRIC_FOLD, never take it.  Nor does a
+//     group with a cut peer link (JR_F_PEER_LINKS): the canonical mail assumes every link delivers.
 //     tests/test_sym_fold.py compares folded runs with step_kernel runs and with the oracle through everything else:
 //     replica state, block tables, leader tables, Instruction streams -- scenario by scenario and over random scripts.
 //     tests/test_sym_abort.py constructs aborts at chosen ticks and CTA positions (the host build logs which site fired,
@@ -634,17 +635,19 @@ __global__ void __launch_bounds__(32 * R, sym_check_ctas(R)) sym_check_kernel(co
   uint4 p0 = make_uint4(0u, 0u, 0u, 0u), p1 = p0, p2 = p0, u0 = p0, u1 = p0, p3 = p0;
   uint2 fc = make_uint2(0u, 0u);
   uint32_t mk = 0, tbase = 0, cnt = 0;
+  unsigned long long cuts = 0;
   const bool in = g < d.G;
   if (in) {
     p0 = d.p0[i]; p1 = d.p1[i]; p2 = d.p2[i]; mk = d.mk[i]; fc = d.fc[i]; tbase = d.tb[g];
     if (p.phases & PH_DRAIN) cnt = d.oc[prv][i];           // mail in flight (the previous tick's outboxes): PH_DRAIN only
+    if (d.links) cuts = d.links[g];                        // JR_F_PEER_LINKS: the fold assumes every link is up
   }
   if (cnt > 0) u0 = unit(0);
   if (cnt > 1) u1 = unit(1);
   const uint32_t meta = p2.w;
   const bool lead = meta_role(meta) == JR_ROLE_LEADER;
-  // roles: one live leader, R-1 live followers of that leader, no queued client requests
-  uint32_t v = !in || !meta_live(meta) || (!lead && meta_role(meta) != JR_ROLE_FOLLOWER) || meta_nq(meta) ? SC_FAIL : 0u;
+  // roles: one live leader, R-1 live followers of that leader, no queued client requests; no cut link
+  uint32_t v = !in || !meta_live(meta) || (!lead && meta_role(meta) != JR_ROLE_FOLLOWER) || meta_nq(meta) || cuts ? SC_FAIL : 0u;
   uint32_t ph_self = 0, ph_f = 0;
   if (lead) {
     // the leader's view of the followers: one progress entry value and mode for all of them

@@ -546,6 +546,52 @@ class RaftApi:
         self._check(self._fn("leader_table")(self._h, buf), "leader_table")
         return [(e.term, e.leader_id, e.commit) for e in buf]
 
+    # -- peer links (F_PEER_LINKS) --------------------------------------------------
+    def set_links(self, cuts, groups: Optional[Sequence[int]] = None):
+        """jr_set_links: the link matrix of groups[i] becomes cuts[i] (see link_cut / partition).  groups None: `cuts`
+        holds one matrix per group.  All or nothing."""
+        cuts = list(cuts)
+        n = len(cuts)
+        if groups is not None and len(groups) != n:
+            raise RaftError(abi.E_INVAL, self._p + "set_links", "groups and cuts differ in length")
+        cs = (C.c_uint64 * max(n, 1))(*cuts)
+        gs = None if groups is None else (C.c_uint32 * max(n, 1))(*groups)
+        self._check(self._fn("set_links")(self._h, gs, cs, C.c_size_t(n)), "set_links")
+
+    def links(self, groups: Optional[Sequence[int]] = None) -> List[int]:
+        """jr_get_links: the link matrices of `groups` (None: every group)."""
+        n = self.n_groups if groups is None else len(groups)
+        gs = None if groups is None else (C.c_uint32 * max(n, 1))(*groups)
+        out = (C.c_uint64 * max(n, 1))()
+        self._check(self._fn("get_links")(self._h, gs, C.c_size_t(n), out), "get_links")
+        return list(out[:n])
+
+    def isolate_leaders(self, salt: int, permille: int) -> int:
+        """jr_isolate_leaders: kill_leaders' groups for the same salt, each live leader cut off both ways (alive)."""
+        v = C.c_uint64(0)
+        self._check(self._fn("isolate_leaders")(self._h, C.c_uint64(salt), C.c_uint32(permille), C.byref(v)),
+                    "isolate_leaders")
+        return v.value
+
+
+def link_cut(n_replicas: int, pairs: Iterable[Tuple[int, int]]) -> int:
+    """The link matrix that cuts mail from node s to node r for every (s, r) in `pairs` (one direction each)."""
+    m = 0
+    for s, r in pairs:
+        if not (1 <= s <= n_replicas and 1 <= r <= n_replicas) or s == r:
+            raise ValueError(f"no link {s} -> {r} in a group of {n_replicas}")
+        m |= 1 << (8 * (r - 1) + (s - 1))
+    return m
+
+
+def partition(n_replicas: int, side: Iterable[int]) -> int:
+    """The link matrix that cuts every link between the nodes in `side` and the others, in both directions."""
+    a = set(side)
+    if not a <= set(range(1, n_replicas + 1)):
+        raise ValueError(f"nodes of a group of {n_replicas} are 1..{n_replicas}")
+    b = set(range(1, n_replicas + 1)) - a
+    return link_cut(n_replicas, [(s, r) for s in a for r in b] + [(s, r) for s in b for r in a])
+
 
 class ReplicaHandle:
     """RaftHandle-style view of one replica (src/raft/mod.rs:437-468)."""
@@ -617,6 +663,9 @@ def _bind(lib: C.CDLL, p: str):
         "engine_save_size": [vp, C.POINTER(C.c_size_t)],
         "engine_save": [vp, C.c_void_p, C.c_size_t],
         "engine_restore": [vp, C.c_void_p, C.c_size_t],
+        "set_links": [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.c_size_t],
+        "get_links": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(C.c_uint64)],
+        "isolate_leaders": [vp, C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)],
     }
     for name, args in sig.items():
         if not hasattr(lib, p + name):   # an older A/B build (JR_ENGINE_LIB): the call site will fail loudly
