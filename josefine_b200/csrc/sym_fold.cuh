@@ -63,12 +63,18 @@ struct SymMail {
   }
 };
 
-// Block-table rows the fold has touched recently, per lane, in SHARED memory: two direct-mapped caches (the leader's
-// table, the followers' identical tables) of SYM_ROWS entries {id, next, token}, laid out [cache][slot][lane] so that a
-// lane's access is one conflict-free 128-bit LDS/STS.  Everything a steady group reads was written a few ticks ago, so
-// after the fill at entry no table READ leaves the SM (rows are still written through to HBM).  (A register shift
-// register costs compare/select chains every tick; local-memory arrays were slower still.)
-constexpr uint32_t SYM_ROWS = 8;
+// Block-table rows the fold has touched recently, per lane, in SHARED memory: two direct-mapped caches of entries
+// {id, next, token}, laid out [slot][lane] so that a lane's access is one conflict-free 128-bit LDS/STS.  Everything a
+// steady group reads was written a few ticks ago, so after the fill at entry no table READ leaves the SM.  (A register
+// shift register costs compare/select chains every tick; local-memory arrays were slower still.)
+//   * the leader's table, SYM_ROWS entries, write-through: the follower lane reads the leader's rows from global memory
+//     whenever a slot may be rewritten in the current tick (fetch_sent);
+//   * the followers' identical tables, SYM_ROWS_F entries, write-back: only the follower lane reads them.  An appended
+//     row stays in the cache, dirty, until a later append evicts it or the launch ends.  It then goes to all R-1 tables
+//     unless the launch's own fused truncation is bound to blank it (evict_f): with jr_set_auto_truncate(margin) most
+//     rows a launch appends lie below the floor it ends with, and are never stored.  16 entries keep a row in the cache
+//     until the commits have passed it by the bench's margin of 8 (the JR_PROFILE build counts drops and write-backs).
+constexpr uint32_t SYM_ROWS = 8, SYM_ROWS_F = 16;
 // The Instruction streams are encoded AS THEY ARE PRODUCED, by the same streaming encoder fsm_flush uses (fsm_enc_push):
 // its state is parked in shared memory between two Instructions, [slot][lane] like the row caches.  (The raw FIFO +
 // fsm_flush round trip of step_kernel cost this kernel a quarter of its instructions and half of its DRAM traffic.)
@@ -77,7 +83,7 @@ constexpr uint32_t SYM_ROWS = 8;
 //   followers f0 = {nrec, seq0, wseq, -}    f1 = {ra.next_id, ra.count, ra.last}   f2 = {ra.stride, -}   (no Notify: pb = 0)
 // seq = seq0 + the lane's Instruction counter (lcnt / fcnt), which lives in a register anyway.
 constexpr uint32_t SYM_ENC_L = 5, SYM_ENC_F = 3;
-constexpr uint32_t SYM_SMEM_UNITS = 2 * SYM_ROWS + SYM_ENC_L + SYM_ENC_F;   // uint4 per lane
+constexpr uint32_t SYM_SMEM_UNITS = SYM_ROWS + SYM_ROWS_F + SYM_ENC_L + SYM_ENC_F;   // uint4 per lane
 // sym2_kernel: TWO lanes per group, in two warps of the same CTA -- one runs the leader's handlers, the other the
 // followers' -- because within a tick the two sides only depend on the mail of the PREVIOUS tick.  One lane per group is
 // latency bound with 3.5 warps per SM sub-partition; two double the warps and halve each warp's serial chain.  The mail goes
@@ -105,6 +111,8 @@ enum : uint32_t {
   SP_EXTEND = 9,       // followers: follower_extend, the R-1 row stores
   SP_ENTER = 10, SP_FILL = 11, SP_LEAVE = 12, SP_TRUNC = 13,   // once per launch: the entry record load, cache fill +
                                                                // encoder init, sym_leave_*, the fused truncation
+  // not phases but counts of the followers' dirty rows (JR_ROLE_FOLLOWER only): [0] = on eviction, [1] = at the exit
+  SP_DROPPED = 14, SP_WRITTEN = 15,
 };
 // The sites at which a lane aborts (SymGroup::fail).  JR_SYM_ABORT_LOG builds only (the host build of tests/emu,
 // tests/test_sym_abort.py) record, per group and lane, the first site that fired and its tick: d.sab[lane * Gp + g] =
@@ -118,6 +126,7 @@ enum : uint32_t {
   SA_HBR = 6,         // leader: leader_tick, HeartbeatResponse{has: false} with a commit above 0
   SA_EXTEND = 7,      // followers: follower_extend, the parent is missing or the window check fails
   SA_PROPOSAL = 8,    // leader: the tick loops, a proposal for a follower
+  SA_DROPPED = 9,     // followers: fetch_f, a cache miss at or below the highest row this launch dropped (evict_f)
 };
 // group s aborts at site `site` (in every other build: exactly the statement `s.abort = true`)
 #ifdef JR_SYM_ABORT_LOG
@@ -125,6 +134,9 @@ enum : uint32_t {
 #else
 #define JR_SYM_ABORT(s, site) ((s).abort = true)
 #endif
+
+// the floor jr_truncate(margin) moves to when the lowest commit is lo (truncate_kernel, engine.cu)
+__device__ __forceinline__ uint32_t trunc_floor(uint32_t lo, uint32_t margin) { return lo > margin ? lo - margin : 0u; }
 
 template <int R>
 struct SymGroup {
@@ -141,6 +153,10 @@ struct SymGroup {
   uint64_t last_hb;
   uint32_t tbase;
   uint32_t flo;                            // lowest id whose row sym_check_kernel found identical in every follower
+  // follower lane, the write-back cache (see above): dirty slots; rows below fbound may be dropped; 1 + the highest row
+  // dropped (0: none); 1 + the highest row below the final floor the followers' tables may hold (entry max key, then
+  // every write-back on eviction)
+  uint32_t fdirty, fbound, fdrop, fhi;
   uint4* rows;                             // this lane's column of the CTA's row caches (see above)
   uint4* enc;                              // this lane's column of the encoder states (see above)
   uint32_t lcnt, fcnt;                     // raw Instructions emitted: leader / each follower
@@ -161,6 +177,7 @@ struct SymGroup {
 #ifdef JR_PROFILE
   long long pt;                            // clock64() at the last phase boundary
   uint32_t prole, pslot;                   // profile role of this lane, phase its cycles go to now
+  uint32_t n_drop[2], n_wb[2];             // the followers' dirty rows dropped / written back: on eviction, at the exit
   // close the current phase (lane 0 of the warp adds the cycles since the last boundary to it), open `slot`; returns the
   // phase it closed, so a nested phase can hand the time back to its caller's
   __device__ __forceinline__ uint32_t phase(uint32_t slot) {
@@ -176,12 +193,15 @@ struct SymGroup {
   __device__ __forceinline__ SymGroup(const Dev& dv, uint32_t g_) : d(dv), g(g_), plane((size_t)R * dv.Gp) {
 #ifdef JR_PROFILE
     pt = 0; prole = JR_ROLE_CANDIDATE; pslot = 0;
+    n_drop[0] = n_drop[1] = n_wb[0] = n_wb[1] = 0;
 #endif
   }
   __device__ __forceinline__ size_t rg(uint32_t r) const { return (size_t)r * d.Gp + g; }
   __device__ __forceinline__ size_t row(uint32_t r, uint32_t bid) const { return table_row(d, plane, bid, rg(r)); }
   __device__ __forceinline__ bool in_window(uint32_t bid) const { return bid - tbase < d.cap; }   // (sym_check_kernel made sure ids stay below 2^31)
-  __device__ __forceinline__ uint4& slot(uint32_t r, uint32_t bid) const { return rows[((r == L ? 0u : SYM_ROWS) + (bid % SYM_ROWS)) * STRIDE]; }
+  __device__ __forceinline__ uint4& slot(uint32_t r, uint32_t bid) const {
+    return rows[(r == L ? bid % SYM_ROWS : SYM_ROWS + bid % SYM_ROWS_F) * STRIDE];
+  }
   __device__ __forceinline__ void cache_put(uint32_t r, uint32_t bid, uint32_t nx, uint64_t tk) const {
     slot(r, bid) = make_uint4(bid, nx, (uint32_t)tk, (uint32_t)(tk >> 32));
   }
@@ -208,7 +228,7 @@ struct SymGroup {
   }
   __device__ __forceinline__ void cache_clear(uint32_t first, uint32_t n) const {
 #pragma unroll
-    for (uint32_t k = 0; k < 2 * SYM_ROWS; ++k)
+    for (uint32_t k = 0; k < SYM_ROWS + SYM_ROWS_F; ++k)
       if (k >= first && k < first + n) rows[k * STRIDE] = make_uint4(ABSENT, ABSENT, 0u, 0u);   // tag ABSENT matches no id
   }
   __device__ __forceinline__ void cache_fill(uint32_t r, uint32_t top) const {   // independent loads, issued together
@@ -230,10 +250,41 @@ struct SymGroup {
     return n != ABSENT;
   }
   // The followers' table, read through the lowest follower's: only rows sym_check_kernel compared across followers (>= flo),
-  // rows this launch wrote to all of them, or ids below the floor (absent everywhere) may be answered that way.
+  // rows this launch wrote to all of them, or ids below the floor (absent everywhere) may be answered that way.  A row
+  // this launch appended is in the cache or was written back -- unless it was dropped: a miss at or below the highest
+  // dropped id aborts (not reached: every such read is at or above the commits the drop bound stays below).
   __device__ __forceinline__ void fetch_f(uint32_t bid, uint32_t& next, uint64_t& tok) {
-    if (in_window(bid) && bid < flo) { JR_SYM_ABORT(*this, SA_FETCH_F); next = ABSENT; tok = 0; return; }
-    fetch(F0, bid, next, tok);
+    next = ABSENT; tok = 0;
+    if (!in_window(bid)) return;
+    if (bid < flo) { JR_SYM_ABORT(*this, SA_FETCH_F); return; }
+    const uint4 e = slot(F0, bid);
+    if (e.x == bid) { next = e.y; tok = (uint64_t)e.z | ((uint64_t)e.w << 32); return; }
+    if (bid < fdrop) { JR_SYM_ABORT(*this, SA_DROPPED); return; }
+    next = __ldcg(d.cnext + row(F0, bid));   // rows written back earlier in this launch by this lane: read them at L2
+    tok = __ldcg(d.ctok + row(F0, bid));
+  }
+  // a dirty row {bid, nx, tk} leaves the followers' cache, on eviction (at = 0) or at the exit (at = 1): dropped if it
+  // lies below `bound`, which never exceeds the floor the launch's fused truncation ends with, else stored to every
+  // follower's table
+  __device__ __forceinline__ void evict_f(const uint4 e, uint32_t bound, int at) {
+    if (e.x < bound) {
+      fdrop = max(fdrop, e.x + 1u);
+#ifdef JR_PROFILE
+      ++n_drop[at];
+#endif
+      return;
+    }
+    const uint64_t tk = (uint64_t)e.z | ((uint64_t)e.w << 32);
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      if ((uint32_t)r != L) {
+        d.cnext[row(r, e.x)] = e.y;
+        d.ctok[row(r, e.x)] = tk;
+      }
+    if (!at) fhi = max(fhi, e.x + 1u);   // (a row written at the exit is at or above the floor: never blanked)
+#ifdef JR_PROFILE
+    ++n_wb[at];
+#endif
   }
   __device__ __forceinline__ bool has_f(uint32_t bid) {
     uint32_t n; uint64_t t;
@@ -493,16 +544,23 @@ struct SymGroup {
   __device__ __forceinline__ void follower_extend(uint32_t bid, uint32_t nx, uint64_t tk) {
     const uint32_t outer = phase(SP_EXTEND);
     if (nx == ABSENT || !has_f(nx) || !in_window(bid)) { JR_SYM_ABORT(*this, SA_EXTEND); return; }   // chain.rs:180-185 Err / window: step_kernel's business
-#pragma unroll
-    for (int r = 0; r < R; ++r)
-      if ((uint32_t)r != L) {
-        d.cnext[row(r, bid)] = nx;
-        d.ctok[row(r, bid)] = tk;
-      }
-    cache_put(F0, bid, nx, tk);
+    // into the write-back cache: the row it evicts leaves now, this one stays dirty
+    uint4& e = slot(F0, bid);
+    const uint32_t k = bid % SYM_ROWS_F;
+    const uint4 old = e;
+    if (((fdirty >> k) & 1u) && old.x != bid) evict_f(old, fbound, 0);
+    e = make_uint4(bid, nx, (uint32_t)tk, (uint32_t)(tk >> 32));
+    fdirty |= 1u << k;
     if (bid > fmaxkey) fmaxkey = bid;
     fhead = bid;                                           // chain.rs:188-190: unconditionally
     phase(outer);
+  }
+  // at the exit of a launch that completes: every dirty row leaves the followers' cache (rows below `floor` are dropped)
+  __device__ __forceinline__ void flush_f(uint32_t floor) {
+#pragma unroll 1
+    for (uint32_t k = 0; k < SYM_ROWS_F; ++k)
+      if ((fdirty >> k) & 1u) evict_f(rows[(SYM_ROWS + k) * STRIDE], floor, 1);
+    fdirty = 0;
   }
   __device__ __forceinline__ void follower_tick(const SymMail& in, SymMail& out) {
     if (in.hb) follower_heartbeat(in, out);
@@ -1023,9 +1081,10 @@ __device__ __forceinline__ void sym_leave_followers(SymGroup<R>& s, const SymMai
 // planes and outbox, the follower lane those of the followers.  Either side may abort: it says so in its mail, the
 // other side sees it one barrier later, and after the last barrier both check the other's final mail, so a group is
 // either left (by both) or not at all.
-// CTAs per SM the register allocation must allow.  The shared memory (480 B per group) caps an SM at 7 CTAs = 448 groups, so
-// on 132 SMs 65,536 groups take two waves whatever the register budget; 4 CTAs (128 registers, next to no spills) run the
-// two waves faster than 7 (72 registers, spilling) run one and a bit.
+// CTAs per SM the register allocation must allow.  The shared memory (608 B per group, 38.9 KB per CTA) caps an SM at 5
+// CTAs = 320 groups, so on 132 SMs 65,536 groups take two waves whatever the register budget; 4 CTAs (128 registers, next
+// to no spills) run exactly two.  (With 480 B per group, before the followers' cache grew to 16 entries, 4 CTAs also ran the
+// two waves faster than 7 at 72 registers, spilling, ran one and a bit.)
 #ifndef JR_SYM2_MINCTAS
 #define JR_SYM2_MINCTAS 4
 #endif
@@ -1048,9 +1107,10 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.n_hb = 0;
   s.last_hb = 0;
   s.share = false;
+  s.fdirty = s.fbound = s.fdrop = 0;
   s.n_app = 1u + p.n_synth;
   s.rows = smem + gi;
-  s.enc = smem + 2 * SYM_ROWS * S + gi;
+  s.enc = smem + (SYM_ROWS + SYM_ROWS_F) * S + gi;
 #ifdef JR_SYM_ABORT_LOG
   s.lane = lead ? 0 : 1;
   s.tick = 0;
@@ -1062,7 +1122,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   s.pslot = SP_ENTER;
   s.pt = clock64();
 #endif
-  s.cache_clear(lead ? 0u : SYM_ROWS, SYM_ROWS);
+  s.cache_clear(lead ? 0u : SYM_ROWS, lead ? SYM_ROWS : SYM_ROWS_F);
   const uint32_t blk = g / GROUPS_PER_CTA;                  // step_kernel's 32-group block of this warp pair
   if (lead && lane == 0 && g < d.Gp) symblk[blk] = 1;      // (cleared below by any lane whose group is not folded)
   SymMail a;
@@ -1078,6 +1138,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
       mail[3 * S] = make_uint4(a.ae_id[1], a.ae_id[2], a.ae_id[3], a.ae_id[4]);
     } else {
       s.cache_fill(s.F0, s.fmaxkey);
+      s.fhi = s.fmaxkey + 1u;
       s.enc_init_followers();
       mail[5 * S] = make_uint4(a.hbr | (a.hbr_has << 1) | (a.ar << 2), a.hbr_commit, a.ar_head, 0u);
     }
@@ -1130,6 +1191,9 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
           SymMail in{}, out{};
           in.hb = ma.x & 1u; in.ae = (ma.x >> 1) & 1u;
           in.hb_commit = ma.y; in.mk = ma.z;
+          // .y (the leader's commit after the last tick; at tick 0 the commit of the Heartbeat in flight) and fcommit
+          // only rise: a floor from them never exceeds the one the launch ends with
+          if (p.trunc) s.fbound = trunc_floor(min(s.fcommit, ma.y), p.trunc_margin);
           if (ma.x & SYM2_IDS) {                           // tick 0: the blocks sym_check_kernel found in the leader's outbox
             const uint4 mb = mail[(2 * (1 - cur) + 1) * S];
             in.ae_nb = (ma.x >> 4) & 15u;
@@ -1165,6 +1229,7 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
     } else {
       last.hbr = lc.x & 1u; last.hbr_has = (lc.x >> 1) & 1u; last.ar = (lc.x >> 2) & 1u;
       last.hbr_commit = lc.y; last.ar_head = lc.z;
+      s.flush_f(p.trunc ? trunc_floor(min(s.fcommit, la.y), p.trunc_margin) : 0u);
       sym_leave_followers(s, last, cur_last, rec);
     }
   }
@@ -1173,12 +1238,16 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
     //              leader's commit after the last tick travels in its last mail
     pair_sync();   // the leader lane's sym_leave may still be reading rows this is about to blank
     if (ok && !lead) {
-      const uint32_t lo = min(s.fcommit, la.y);
-      const uint32_t floor = lo > p.trunc_margin ? lo - p.trunc_margin : 0u;
+      const uint32_t floor = trunc_floor(min(s.fcommit, la.y), p.trunc_margin);
       if (floor > s.tbase) {
-        for (uint32_t b = s.tbase; b < floor && b - s.tbase < d.cap; ++b)
+        // the followers' rows from fhi up were absent at entry (no replica holds a row above its max key, DESIGN.md
+        // §3b) and this launch stored none of them: above fhi only the leader's.  (Below it every table, the leader's
+        // too, so that a warp whose groups have their leaders on different replicas still stores whole lines.)
+        const uint32_t ftop = min(floor, s.fhi);
+        for (uint32_t b = s.tbase; b < ftop; ++b)
 #pragma unroll
           for (int r = 0; r < R; ++r) d.cnext[s.row(r, b)] = ABSENT;
+        for (uint32_t b = ftop; b < floor && b - s.tbase < d.cap; ++b) d.cnext[s.row(s.L, b)] = ABSENT;
         d.tb[g] = floor;
       }
     }
@@ -1192,6 +1261,12 @@ __global__ void __launch_bounds__(2 * SYM2_GROUPS, JR_SYM2_MINCTAS) sym2_kernel(
   }
 #ifdef JR_PROFILE
   s.phase(SP_TRUNC);
+  if (!lead)
+    for (int at = 0; at < 2; ++at) {
+      unsigned long long* c = jr_prof_smem() + ((w * 3 + JR_ROLE_FOLLOWER) * 16) * 2 + at;
+      atomicAdd(c + SP_DROPPED * 2, (unsigned long long)s.n_drop[at]);
+      atomicAdd(c + SP_WRITTEN * 2, (unsigned long long)s.n_wb[at]);
+    }
   __syncthreads();
   if (d.prof)
     for (uint32_t i = threadIdx.x; i < 4 * 3 * 16 * 2; i += blockDim.x) {

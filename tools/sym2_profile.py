@@ -66,6 +66,14 @@ def main():
         for s, name in LAUNCH.items():
             if cnt(s):
                 print(f"  {name:38s} {cyc(s) / warps:8.0f}")
+    # the followers' write-back row cache (SP_DROPPED / SP_WRITTEN): dirty rows per group-launch, [0] evicted by an
+    # append, [1] left at the exit.  Nearly every eviction should be a drop; many write-backs mean the cache is too small
+    # for the truncation margin.
+    gl = G * launches
+    row = lambda s: (buf[(FOLLOWER * 16 + s) * 2] / gl, buf[(FOLLOWER * 16 + s) * 2 + 1] / gl)
+    (de, dx), (we, wx) = row(14), row(15)
+    print(f"== followers' dirty rows per group-launch: on eviction {de:.2f} dropped / {we:.2f} written back; "
+          f"at the exit {dx:.2f} dropped / {wx:.2f} written back")
 
 
 if __name__ == "__main__":
