@@ -40,6 +40,7 @@
  *   jr_group_export / jr_group_import <- no reference API: reassigning a group to another engine
  *   jr_set_links / jr_get_links / jr_isolate_leaders <- no reference API: a tcp.rs connection that delivers nothing
  *                         (deviation D8)
+ *   jr_get_link_queues <- no reference API: the depth of send_task's per-peer channel (tcp.rs:63), D8
  *
  * One engine = G independent Raft groups x R replicas, all resident in one GPU's
  * HBM.  The reference is one group, one node per process; the group dimension is
@@ -74,10 +75,13 @@
  *       must then lie in [floor, floor + chain_capacity).  Removed keys read as absent, exactly as
  *       if sled had lost them (has() false, range() skips them).  An engine that never calls
  *       jr_truncate behaves as before (floor 0).
- *   D8  peer-link cuts (JR_F_PEER_LINKS): mail over a cut link is DROPPED at delivery.  The reference
- *       keeps it: while a TCP connect fails, the message stays in the sender's channel and goes out
- *       once the connection is back (tcp.rs:110-135, connect_and_send).  Delayed delivery is not
- *       modelled; the schedule already drops mail that is not delivered in the next step.
+ *   D8  peer-link cuts (JR_F_PEER_LINKS): without JR_F_LINK_QUEUES, mail over a cut link is DROPPED at delivery.
+ *       The reference keeps it: while a TCP connect fails, the message waits in the sender's bounded channel
+ *       (mpsc::channel(1000), tcp.rs:63; try_send drops only the new message once it is full, tcp.rs:90-92) and goes
+ *       out, in order, once the connection is back (tcp.rs:110-135, connect_and_send).  With JR_F_LINK_QUEUES the
+ *       engine does the same with a bound of JR_LINK_QUEUE_MSGS messages per directed link: cut mail is queued and
+ *       replayed at the first delivery after the heal (see "link queues" below).  The reconnect backoff
+ *       (tcp.rs:115-129) is not modelled: queued mail goes out at the first delivering step after the heal.
  *
  * All structs are plain data, little endian, naturally aligned.  No callbacks.
  * Buffers passed to jr_step are HOST memory owned by the caller.
@@ -103,6 +107,8 @@ extern "C" {
 #define JR_CLIENT_QUEUE_CAP 4u    /* queued_reqs bound per replica (reference: Vec)  */
 #define JR_NOTIFY_RUNS 8u         /* pending-notification runs per replica with JR_F_CLIENT_RESPONSES
                                    * (reference: the Driver's unbounded HashMap, fsm.rs:36,78-81) */
+#define JR_LINK_QUEUE_MSGS 8u     /* Messages one directed link holds while it is cut, with JR_F_LINK_QUEUES
+                                   * (reference: mpsc::channel::<Message>(1000), tcp.rs:63) */
 
 /* ---- status codes (API misuse / resources; never consensus outcomes) ---- */
 typedef enum jr_status {
@@ -170,9 +176,12 @@ enum {
                                           * identical either way -- the flag exists for A/B measurements and tests      */
   JR_F_CLIENT_RESPONSES = 1u << 5,       /* every drain also runs fsm::Driver's notification map on the device and returns the
                                           * ClientResponses it produces (jr_fsm_responses).  Requires JR_F_CAPTURE_FSM */
-  JR_F_PEER_LINKS = 1u << 6              /* each group keeps a link matrix: jr_set_links / jr_get_links / jr_isolate_leaders
+  JR_F_PEER_LINKS = 1u << 6,             /* each group keeps a link matrix: jr_set_links / jr_get_links / jr_isolate_leaders
                                           * cut and heal the connections between its replicas (D8).  Without the flag those
                                           * calls return JR_E_INVAL and nothing is allocated */
+  JR_F_LINK_QUEUES = 1u << 7             /* mail over a cut link is queued (up to JR_LINK_QUEUE_MSGS per link) and delivered
+                                          * when the link heals, instead of dropped (D8; jr_get_link_queues).  Requires
+                                          * JR_F_PEER_LINKS; without the flag nothing is allocated */
 };
 
 /* ---- configuration (RaftConfig, src/raft/config.rs:14-41, batched) --------- */
@@ -711,7 +720,8 @@ jr_status jr_kill_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64
  * delivered.  A cut is directional (a symmetric partition sets both bits).  Bits on the diagonal (r == s) and bits that
  * name a node above n_replicas are refused.  A new engine, and every jr_engine_reset, starts fully connected (all zero).
  *   What is dropped: at delivery (schedule item 1 of jr_step_args) receiver r skips every unit of a sender whose bit is
- *   set in its row -- mail addressed to it and Peers broadcasts alike.  The mail is dropped, not delayed (D8).
+ *   set in its row -- mail addressed to it and Peers broadcasts alike.  The mail is dropped, not delayed (D8), unless
+ *   the engine has JR_F_LINK_QUEUES (see "link queues" below).
  *   What is not affected: emission (the stream digests, n_msgs and jr_step's out_msgs hold every Message emitted);
  *   jr_step's inject[] entries (the host is the network for injected mail); proposals, Tick, jr_set_alive, restarts,
  *   truncation, compaction and verification.  A cut-off replica is still alive, so it still holds jr_truncate's floor
@@ -733,6 +743,36 @@ jr_status jr_get_links(jr_engine* e, const uint32_t* groups, size_t n, uint64_t*
  * and from each live leader is cut (ORed into the matrix): the leader stays alive but reaches no one and hears no one.
  * *n_isolated = the selected groups that had a live leader (also at n_replicas = 1, where there is no link to cut). */
 jr_status jr_isolate_leaders(jr_engine* e, uint64_t salt, uint32_t permille, uint64_t* n_isolated);
+
+/*
+ * ---- link queues (JR_F_LINK_QUEUES, requires JR_F_PEER_LINKS; deviation D8) -------------------------------------------
+ * Normative:
+ * Each directed link s -> r of a group has a FIFO of at most JR_LINK_QUEUE_MSGS Messages.
+ *   Queueing: at a delivery (schedule item 1 of jr_step_args) where receiver r skips sender s because bit 8*(r-1)+(s-1)
+ *   of the matrix is set, every Message of s's previous-step mail that r would have received (Peer(r) mail and Peers
+ *   broadcasts) is appended to the queue of s -> r, in order, while it holds fewer than JR_LINK_QUEUE_MSGS; once it is
+ *   full, later Messages are dropped (try_send on a full channel, tcp.rs:90-92).  Every Message counts as one: a no-op
+ *   HeartbeatResponse too, and each of the R-1 copies of a seek_election VoteRequest (candidate.rs:30-37); if only j of
+ *   its k copies fit, j are kept.  This happens whether r is alive, silenced or faulted.  A step without
+ *   JR_STEP_DELIVER queues nothing: its mail is dropped like all undelivered mail.
+ *   Replay: at the first delivery to r after s -> r is up again while its queue is not empty, the queued Messages are
+ *   delivered first, oldest first, in sender s's place of the ascending-sender order; s's previous-step mail follows.
+ *   The queue is then empty.  A silenced or faulted r loses them, as it loses all mail.
+ *   jr_node_restart / jr_node_restart_many of node n empty every queue FROM n (a new process has new channels); queues
+ *   TO n stay.  jr_engine_reset empties every queue.  jr_set_alive, jr_kill_leaders, jr_isolate_leaders, jr_truncate,
+ *   jr_compact and jr_verify_groups do not touch them.  jr_engine_save / jr_engine_restore and group images carry them
+ *   (jr_group_import gives the slot the image's queues; jr_group_export leaves the source slot's as they were);
+ *   jr_engine_restore and jr_group_import refuse queue depths above JR_LINK_QUEUE_MSGS, queues larger than a link's
+ *   storage and non-empty masks that do not match the depths, before anything reaches the device.
+ *   Emission is unchanged: stream digests, n_msgs, out_msgs and jr_state_digest see neither queueing nor replay.
+ *   A replay is a burst: each queued HeartbeatResponse may make a leader replicate to every peer within the same step,
+ *   so size mailbox_units for it; a replica that emits more faults with JR_FAULT_ENGINE_MAILBOX_OVERFLOW, as always.
+ *   A group with a cut link or a non-empty queue does not take the symmetric-group fold.
+ */
+/* depths[64*i + 8*(r-1) + (s-1)] = Messages queued on link s -> r of groups[i] (other bytes 0).  groups == NULL:
+ * n == n_groups, every group.  Synchronous.  JR_E_INVAL (nothing written) for a group out of range or named twice, or on
+ * an engine created without JR_F_LINK_QUEUES. */
+jr_status jr_get_link_queues(jr_engine* e, const uint32_t* groups, size_t n, uint8_t* depths);
 
 /* ---- leader announce ------------------------------------------------------- */
 /* Writes n_groups entries to DEVICE memory `dev_out` (for a collective) */

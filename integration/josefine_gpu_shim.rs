@@ -203,6 +203,9 @@ extern "C" {
     fn jr_get_links(e: *mut c_void, groups: *const u32, n: usize, out: *mut u64) -> c_int;
     #[allow(dead_code)]
     fn jr_isolate_leaders(e: *mut c_void, salt: u64, permille: u32, n_isolated: *mut u64) -> c_int;
+    // link queues (JR_F_LINK_QUEUES): depths[64*i + 8*(r-1) + (s-1)] = Messages queued on link s -> r of groups[i]
+    #[allow(dead_code)]
+    fn jr_get_link_queues(e: *mut c_void, groups: *const u32, n: usize, depths: *mut u8) -> c_int;
 }
 
 /// jr_verify_report: what one jr_verify_groups call checked, and its findings per kind.

@@ -13,6 +13,7 @@ MAX_AE_BLOCKS = 5
 MAX_NODE_ID = 65534
 CLIENT_QUEUE_CAP = 4
 NOTIFY_RUNS = 8           # JR_NOTIFY_RUNS: pending-notification runs per replica (F_CLIENT_RESPONSES)
+LINK_QUEUE_MSGS = 8       # JR_LINK_QUEUE_MSGS: Messages a cut link holds (F_LINK_QUEUES)
 
 # jr_status
 OK, E_INVAL, E_NOMEM, E_CUDA, E_CAPACITY, E_UNKNOWN_NODE, E_NO_DEVICE = range(7)
@@ -53,6 +54,7 @@ F_STREAM_DIGEST = 1 << 3
 F_NO_SYMMETRIC_FOLD = 1 << 4
 F_CLIENT_RESPONSES = 1 << 5
 F_PEER_LINKS = 1 << 6
+F_LINK_QUEUES = 1 << 7
 
 # step flags
 STEP_DELIVER = 1 << 0
@@ -217,7 +219,7 @@ ENGINE_SYMBOLS = [
     "jr_set_alive", "jr_kill_leaders", "jr_leader_table_device", "jr_leader_table", "jr_leader_table_async", "jr_leader_table_wait",
     "jr_election_timeout", "jr_fsm_records_async", "jr_fsm_records_wait", "jr_fsm_responses", "jr_fsm_expand", "jr_fsm_fold", "jr_fsm_fold_mt", "jr_query_many",
     "jr_chain_read_many", "jr_truncate", "jr_set_auto_truncate", "jr_host_alloc", "jr_host_free", "jr_node_restart", "jr_chain_export_many", "jr_node_restart_many", "jr_verify_groups", "jr_group_export", "jr_group_import", "jr_engine_save_size", "jr_engine_save", "jr_engine_restore",
-    "jr_set_links", "jr_get_links", "jr_isolate_leaders",
+    "jr_set_links", "jr_get_links", "jr_isolate_leaders", "jr_get_link_queues",
 ]
 
 

@@ -70,7 +70,9 @@ __device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
 // was added; the other sizes keep their natural allocation.
 constexpr int step_min_ctas(int R) { return (R == 4 || R == 5) ? 4 : 1; }
 
-template <int R, bool SORTED>
+// QUEUES: the engine has JR_F_LINK_QUEUES (cut mail is queued and replayed, raft_device.cuh); a separate instantiation,
+// so the other engines' kernel keeps its code and registers.
+template <int R, bool SORTED, bool QUEUES = false>
 __global__ void __launch_bounds__(32 * R, step_min_ctas(R)) step_kernel(const Dev d, const StepParams p0) {
   JR_DYN_SMEM(uint4, smem);
   const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31u;
@@ -129,7 +131,7 @@ __global__ void __launch_bounds__(32 * R, step_min_ctas(R)) step_kernel(const De
   L.mk_in = reinterpret_cast<uint16_t*>(L.cout + R * 32);
   L.mk_out = L.mk_in + R * R * 32;
   L.Us = d.Us; L.W = d.W; L.lane = lane;
-  Replica<R, SORTED> rep(d, L, r, g);
+  Replica<R, SORTED, QUEUES> rep(d, L, r, g);
   rep.now = p.now;
   rep.cur = p.cur;
   rep.load(p.phases & PH_RESET_OUT, p.phases & PH_RESET_FSM, part != 0);
@@ -504,6 +506,31 @@ __global__ void links_gather_kernel(const Dev d, const uint32_t* groups, uint32_
   if (k < n) out[k] = d.links[groups[k]];
 }
 
+// jr_get_link_queues: depths[64*k + 8*r + s] = Messages queued on link s -> r of groups[k] (groups null: group k).
+__global__ void link_queues_gather_kernel(const Dev d, const uint32_t* groups, uint32_t n, uint8_t* depths) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t g = groups ? groups[k] : k;
+  uint8_t* o = depths + 64 * (size_t)k;
+  for (uint32_t x = 0; x < 64; ++x) o[x] = 0;
+  for (uint32_t r = 0; r < d.R; ++r)
+    for (uint32_t s = 0; s < d.R; ++s)
+      if (s != r) o[8 * r + s] = (uint8_t)(d.lqc[((size_t)lq_slot(r, s) * d.R + r) * d.Gp + g] & 255u);
+}
+
+// After node_restart_kernel emptied the queues from the restarted nodes: each named group's non-empty mask, from its
+// counts (a separate launch, so that requests for several nodes of one group never race on the mask).
+__global__ void link_queues_mask_kernel(const Dev d, const jr_persisted_chain* reqs, uint32_t n) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t g = reqs[k].group;
+  unsigned long long m = 0;
+  for (uint32_t r = 0; r < d.R; ++r)
+    for (uint32_t s = 0; s < d.R; ++s)
+      if (s != r && d.lqc[((size_t)lq_slot(r, s) * d.R + r) * d.Gp + g]) m |= 1ull << (8 * r + s);
+  d.lqm[g] = m;   // (every request of group g stores the same value)
+}
+
 __global__ void set_alive_kernel(const Dev d, uint32_t g, uint32_t r, int alive) {
   const size_t i = (size_t)r * d.Gp + g;
   const uint32_t m = d.p2[i].w;
@@ -691,6 +718,9 @@ __global__ void node_restart_kernel(const Dev d, uint64_t now, const jr_persiste
   d.mk[i] = mk;
   d.oc[0][i] = 0;
   d.oc[1][i] = 0;
+  if (d.lqc)   // a new process has new channels: the queues FROM this node are gone (link_queues_mask_kernel follows)
+    for (uint32_t q = 0; q < d.R; ++q)
+      if (q != r) d.lqc[((size_t)lq_slot(q, r) * d.R + q) * d.Gp + g] = 0;
   if (rm) {
     const uint32_t pos = d.fc[i].y;
     uint4 m = rm[i];
@@ -1436,17 +1466,25 @@ static jr_status dalloc(jr_engine* e, T** p, size_t n) {
     default: { constexpr int RR = 8; CALL; } break; \
   }
 
+// (R = 1 has no links: its engines never need the queue instantiation)
 template <int R>
 static void launch_step_r(jr_engine* e, const StepParams& p, bool sorted, uint32_t grid, size_t smem) {
   auto kfn = sorted ? step_kernel<R, true> : step_kernel<R, false>;
+  if constexpr (R > 1)
+    if (e->d.lq) kfn = sorted ? step_kernel<R, true, true> : step_kernel<R, false, true>;
   JR_LAUNCH_SMEM(kfn, grid, 32 * R, smem, e->stream, e->d, p);
 }
 
 template <int R>
-static cudaError_t step_smem_attr_r(int smem) {
+static cudaError_t step_smem_attr_r(int smem, bool queues) {
   cudaError_t a = cudaFuncSetAttribute(step_kernel<R, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (a != cudaSuccess) return a;
-  return cudaFuncSetAttribute(step_kernel<R, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (a == cudaSuccess) a = cudaFuncSetAttribute(step_kernel<R, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if constexpr (R > 1)
+    if (queues && a == cudaSuccess) {
+      a = cudaFuncSetAttribute(step_kernel<R, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      if (a == cudaSuccess) a = cudaFuncSetAttribute(step_kernel<R, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    }
+  return a;
 }
 
 #ifndef JR_EMU
@@ -1611,6 +1649,10 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
     set_err("JR_F_CLIENT_RESPONSES requires JR_F_CAPTURE_FSM");
     return JR_E_INVAL;
   }
+  if ((cfg->flags & JR_F_LINK_QUEUES) && !(cfg->flags & JR_F_PEER_LINKS)) {
+    set_err("JR_F_LINK_QUEUES requires JR_F_PEER_LINKS");
+    return JR_E_INVAL;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     set_err("no CUDA device; this library has no CPU fallback");
@@ -1667,6 +1709,12 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
   A(e->symblk, d.Gp / GROUPS_PER_CTA);
   A(e->symrec, (size_t)sym_record_words(d.R) * d.Gp);
   if (d.flags & JR_F_PEER_LINKS) A(d.links, d.Gp);   // (padded groups too: step_kernel's lanes read their row)
+  if (d.flags & JR_F_LINK_QUEUES) {                   // (R = 1: one slot, never used, so that every pointer is set)
+    const size_t slots = std::max<uint32_t>(d.R - 1, 1u);
+    A(d.lq, (size_t)LQ_UNITS * slots * plane);
+    A(d.lqc, slots * plane);
+    A(d.lqm, d.Gp);
+  }
   if (d.flags & JR_F_CAPTURE_FSM) {
     const size_t reps = (size_t)cfg->n_groups * cfg->n_replicas;   // default: 2 per replica, but never less than a small engine's whole FIFO space
     const size_t want = cfg->fsm_host_records ? cfg->fsm_host_records
@@ -1737,7 +1785,7 @@ jr_status jr_engine_create(const jr_config* cfg, jr_engine** out) {
   {
     const int smem = (int)step_smem_bytes(d);
     cudaError_t aerr = cudaSuccess;
-    DISPATCH_R(d.R, (aerr = step_smem_attr_r<RR>(smem)));
+    DISPATCH_R(d.R, (aerr = step_smem_attr_r<RR>(smem, d.lq != nullptr)));
     if (aerr == cudaSuccess) aerr = cudaHostAlloc((void**)&e->h_scatter, sizeof(uint32_t), cudaHostAllocMapped);
     if (aerr == cudaSuccess) *e->h_scatter = 0;
     if (aerr == cudaSuccess) aerr = cudaHostGetDevicePointer((void**)&e->d.hscat, (void*)e->h_scatter, 0);
@@ -1814,6 +1862,12 @@ jr_status jr_engine_reset(jr_engine* e) {
     CK(cudaMemsetAsync(e->rp.pnc, 0, ((plane + 3) / 4 + plane) * sizeof(uint4), e->stream));
   e->resp_b = -1;
   if (d.links) CK(cudaMemsetAsync(d.links, 0, (size_t)d.Gp * sizeof(unsigned long long), e->stream));   // fully connected
+  if (d.lq) {   // every link queue empty (the units too: a checkpoint's bytes depend only on what the engine did)
+    const size_t slots = std::max<uint32_t>(d.R - 1, 1u);
+    CK(cudaMemsetAsync(d.lq, 0, (size_t)LQ_UNITS * slots * plane * sizeof(uint4), e->stream));
+    CK(cudaMemsetAsync(d.lqc, 0, slots * plane * sizeof(uint32_t), e->stream));
+    CK(cudaMemsetAsync(d.lqm, 0, (size_t)d.Gp * sizeof(unsigned long long), e->stream));
+  }
   JR_LAUNCH(init_kernel, (unsigned)((plane + 255) / 256), 256, e->stream, d);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -2989,6 +3043,10 @@ jr_status jr_node_restart_many(jr_engine* e, uint64_t now_ms, const jr_persisted
   JR_LAUNCH(node_restart_kernel, (unsigned)((n + 127) / 128), 128, e->stream, d, now_ms, (const jr_persisted_chain*)base,
             (uint32_t)n, (const jr_block*)(base + o_blk), e->rp.rm);
   CK(cudaGetLastError());
+  if (d.lqm) {
+    JR_LAUNCH(link_queues_mask_kernel, (unsigned)((n + 127) / 128), 128, e->stream, d, (const jr_persisted_chain*)base, (uint32_t)n);
+    CK(cudaGetLastError());
+  }
   CK(cudaStreamSynchronize(e->stream));
   return JR_OK;
 }
@@ -3137,7 +3195,28 @@ std::vector<PlaneDesc> engine_planes(jr_engine* e) {
   }
   if (d.links)   // the link matrices (JR_F_PEER_LINKS only, for the same reason)
     v.push_back({d.links, (size_t)d.Gp * sizeof(unsigned long long), Carry::WORDS, 2, 1, true});
+  if (d.lq) {    // the link queues (JR_F_LINK_QUEUES only): non-empty masks, counts, units
+    const uint32_t slots = std::max<uint32_t>(d.R - 1, 1u);
+    v.push_back({d.lqm, (size_t)d.Gp * sizeof(unsigned long long), Carry::WORDS, 2, 1, true});
+    v.push_back({d.lqc, plane * slots * sizeof(uint32_t), Carry::WORDS, 1, slots});
+    v.push_back({d.lq, plane * slots * LQ_UNITS * sizeof(uint4), Carry::WORDS, 4, slots * LQ_UNITS});
+  }
   return v;
+}
+
+// One group's link queues, as a checkpoint or an image holds them: every depth <= JR_LINK_QUEUE_MSGS, every queue within
+// its link's LQ_UNITS, units exactly when there are Messages, and the non-empty mask holding exactly the non-empty links.
+// count[r][s] = the count word of link s -> r (replica indices).
+bool link_queues_valid(uint32_t R, uint64_t mask, const uint32_t (*count)[JR_MAX_REPLICAS]) {
+  uint64_t want = 0;
+  for (uint32_t r = 0; r < R; ++r)
+    for (uint32_t s = 0; s < R; ++s) {
+      if (s == r) continue;
+      const uint32_t c = count[r][s], nm = c & 255u, nu = c >> 8;
+      if (nm > JR_LINK_QUEUE_MSGS || nu > LQ_UNITS || (nm == 0) != (nu == 0)) return false;
+      if (nm) want |= 1ull << (8 * r + s);
+    }
+  return mask == want;
 }
 
 struct Segment { void* p; size_t n; };
@@ -3193,6 +3272,28 @@ jr_status jr_engine_restore(jr_engine* e, const void* buf, size_t bytes) {
     set_err("checkpoint does not match this engine's configuration");
     return JR_E_INVAL;
   }
+  if (e->d.lq) {   // the link queues, checked before anything reaches the device
+    const Dev& d = e->d;
+    const unsigned char *qm = nullptr, *qc = nullptr;
+    const unsigned char* at = (const unsigned char*)buf + sizeof h;
+    for (const Segment& sg : save_segments(e)) {
+      if (sg.p == d.lqm) qm = at;
+      if (sg.p == d.lqc) qc = at;
+      at += sg.n;
+    }
+    for (uint32_t g = 0; g < d.Gp; ++g) {
+      uint64_t m;
+      memcpy(&m, qm + 8 * (size_t)g, 8);
+      uint32_t count[JR_MAX_REPLICAS][JR_MAX_REPLICAS] = {};
+      for (uint32_t r = 0; r < d.R; ++r)
+        for (uint32_t s = 0; s < d.R; ++s)
+          if (s != r) memcpy(&count[r][s], qc + 4 * (((size_t)lq_slot(r, s) * d.R + r) * d.Gp + g), 4);
+      if (!link_queues_valid(d.R, m, count)) {
+        set_err("checkpoint: the link queues of group %u are inconsistent or exceed their bounds", g);
+        return JR_E_INVAL;
+      }
+    }
+  }
   CK(cudaSetDevice(e->cfg.device));
   jr_status st = jr_engine_sync(e);
   if (st != JR_OK) return st;
@@ -3227,6 +3328,7 @@ struct ImgLayout {
   std::vector<ImgPlane> planes;   // the WORDS planes, in list order
   uint32_t words = 0, rec_units = 0;
   uint32_t w_fc = 0, w_tb = 0, w_pnc = ~0u;   // word offsets inside a record's planes
+  uint32_t w_lqm = ~0u, w_lqc = ~0u;          // (JR_F_LINK_QUEUES)
 };
 ImgLayout img_layout(jr_engine* e) {
   ImgLayout L;
@@ -3235,6 +3337,8 @@ ImgLayout img_layout(jr_engine* e) {
     if (pd.p == e->d.fc) L.w_fc = L.words;
     if (pd.p == e->d.tb) L.w_tb = L.words;
     if (pd.p == e->rp.pnc) L.w_pnc = L.words;
+    if (pd.p == e->d.lqm) L.w_lqm = L.words;
+    if (pd.p == e->d.lqc) L.w_lqc = L.words;
     L.planes.push_back(ImgPlane{(uint32_t*)pd.p, pd.words, pd.depth, pd.per_group ? 1u : 0u});
     L.words += pd.words * pd.depth;
   }
@@ -3398,6 +3502,18 @@ jr_status jr_group_import(jr_engine* e, const uint32_t* slots, size_t n, const v
     at += (unsigned long long)c.x + c.y + 2ull * c.z + 2ull * c.w;
   }
   if (fixed + at != units) { set_err("truncated image"); return JR_E_INVAL; }
+  if (L.w_lqm != ~0u)   // the link queues: each group's mask (carried in its first replica's record) against its counts
+    for (size_t j = 0; j < n; ++j) {
+      const uint64_t m = (uint64_t)word(j, L.w_lqm) | ((uint64_t)word(j, L.w_lqm + 1) << 32);
+      uint32_t count[JR_MAX_REPLICAS][JR_MAX_REPLICAS] = {};
+      for (uint32_t r = 0; r < d.R; ++r)
+        for (uint32_t s = 0; s < d.R; ++s)
+          if (s != r) count[r][s] = word((size_t)r * n + j, L.w_lqc + lq_slot(r, s));
+      if (!link_queues_valid(d.R, m, count)) {
+        set_err("group %zu of the image: link queues inconsistent or beyond their bounds", j);
+        return JR_E_INVAL;
+      }
+    }
   for (size_t t = 0; t < reps; ++t) {   // then the rows: ascending, inside the window, below 2^31 (D4, D7)
     const uint32_t rows = unit(t * L.rec_units).x;
     const uint64_t lo = floor[t % n];
@@ -3516,6 +3632,25 @@ jr_status jr_get_links(jr_engine* e, const uint32_t* groups, size_t n, uint64_t*
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out, dout, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
   }
+  CK(cudaStreamSynchronize(e->stream));
+  return JR_OK;
+}
+
+jr_status jr_get_link_queues(jr_engine* e, const uint32_t* groups, size_t n, uint8_t* depths) {
+  if (!e || (n && !depths)) return JR_E_INVAL;
+  if (!e->d.lq) { set_err("jr_get_link_queues: engine created without JR_F_LINK_QUEUES"); return JR_E_INVAL; }
+  jr_status st = links_check_groups(e, groups, n, "jr_get_link_queues");
+  if (st != JR_OK) return st;
+  if (n == 0) return JR_OK;
+  CK(cudaSetDevice(e->cfg.device));
+  const size_t o_grp = n * 64;   // the depths, then the group list
+  if ((st = many_reserve(e, o_grp + (groups ? n * sizeof(uint32_t) : 0))) != JR_OK) return st;
+  uint8_t* dout = (uint8_t*)e->many_buf;
+  uint32_t* dgroups = groups ? (uint32_t*)(dout + o_grp) : nullptr;
+  if (groups) CK(cudaMemcpyAsync(dgroups, groups, n * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+  JR_LAUNCH(link_queues_gather_kernel, (unsigned)((n + 127) / 128), 128, e->stream, e->d, (const uint32_t*)dgroups, (uint32_t)n, dout);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(depths, dout, n * 64, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return JR_OK;
 }

@@ -66,12 +66,22 @@ struct Dev {
                                    // [1] task ticket counter of the running step launch (both zeroed per launch)
   uint32_t* done;                  // [CTA-sized group block]: epoch + parts finished (split launches, see step_kernel)
   unsigned long long* links;       // JR_F_PEER_LINKS, else null: [group] link matrix, bit 8*(r-1)+(s-1) = mail s -> r is cut
+  // JR_F_LINK_QUEUES, else null (DESIGN.md section 3g, "Link queues").  Receiver r owns its incoming queues; slot = the
+  // sender's place among r's R-1 peers (lq_slot):
+  uint4* lq;                       // queued units [unit * (R-1) + slot][replica r][group], LQ_UNITS per link
+  uint32_t* lqc;                   // [slot][replica r][group]: Messages | units << 8 queued on the link
+  unsigned long long* lqm;         // [group]: non-empty mask in the matrix's layout (receiver r writes only byte r)
   unsigned long long* prof;        // JR_PROFILE builds: cycle counters [role 3][slot 16] x {cycles, count}
 #ifdef JR_SYM_ABORT_LOG
   uint32_t* sab;                   // [lane 2][group]: the fold's first abort site | tick << 8 (sym_fold.cuh, SA_*)
 #endif
   uint64_t seed, goff;
 };
+
+// Link queues (JR_F_LINK_QUEUES): units one directed link can hold -- JR_LINK_QUEUE_MSGS AppendEntries with all blocks.
+constexpr uint32_t LQ_UNITS = JR_LINK_QUEUE_MSGS * (1u + JR_MAX_AE_BLOCKS);
+// Sender s's slot among the R-1 incoming links of receiver r (replica indices, s != r).
+__host__ __device__ inline uint32_t lq_slot(uint32_t r, uint32_t s) { return s - (s > r ? 1u : 0u); }
 
 // A replica's meta word, P2.w: role (bits 0-7), fault (8-15), pre-vote mask (16-23), queued client requests (24-26),
 // dead (27), commit key (28).
@@ -380,7 +390,8 @@ __device__ __noinline__ void fsm_flush(const uint4* raw0, uint32_t n_raw, uint32
   *fc = c;
 }
 
-template <int R, bool SORTED = false>
+// QUEUES: the engine has JR_F_LINK_QUEUES (a second instantiation of step_kernel; the other kernels never set it).
+template <int R, bool SORTED = false, bool QUEUES = false>
 struct Replica {
   const Dev& d;
   const Local& L;
@@ -406,6 +417,7 @@ struct Replica {
   //  product kernel six registers)
   uint32_t mko[R];       // delivery index of this tick's outbox, one mask per receiver (see Local::mk_out)
   uint32_t cut;          // senders (bit s = replica index s) whose mail this replica does not receive (JR_F_PEER_LINKS)
+  uint32_t qne;          // QUEUES: senders whose link to me has queued mail (my byte of d.lqm)
 
   __device__ __forceinline__ Replica(const Dev& dv, const Local& lv, uint32_t r_, uint32_t g_)
       : d(dv), L(lv), r(r_), g(g_), rg((size_t)r_ * dv.Gp + g_), plane((size_t)R * dv.Gp) {}
@@ -426,6 +438,7 @@ struct Replica {
     maxkey = d.mk[rg];
     tbase = d.tb[g];
     cut = d.links ? (uint32_t)(d.links[g] >> (8u * r)) & 255u : 0u;   // this replica's row; constant within a launch
+    if constexpr (QUEUES) qne = (uint32_t)(d.lqm[g] >> (8u * r)) & 255u;
     hbtime = 0;
 #pragma unroll
     for (int i = 0; i < (R < 3 ? 3 : R); ++i) ph[i] = 0;
@@ -618,6 +631,63 @@ struct Replica {
     if (u < L.Us) return L.in[(u * R + s_) * 32 + L.lane];
     return __ldcg(d.ob[1 - cur] + ((size_t)u * R + s_) * d.Gp + g);  // spilled unit: L2, never a stale L1 line
   }
+  // ---- link queues (QUEUES only; DESIGN.md section 3g).  A mail source is a sender index s < R (its mailbox) or R + s
+  // (the queue of link s -> me).
+  __device__ __forceinline__ size_t lq_count_at(uint32_t s_) const { return ((size_t)lq_slot(r, s_) * R + r) * d.Gp + g; }
+  __device__ __forceinline__ uint4* lq_unit(uint32_t s_, uint32_t u) const {
+    return d.lq + ((size_t)(u * (R - 1) + lq_slot(r, s_)) * R + r) * d.Gp + g;
+  }
+  __device__ __forceinline__ uint4 mail_unit(uint32_t src, uint32_t u) const {
+    if constexpr (QUEUES)
+      if (src >= (uint32_t)R) return *lq_unit(src - R, u);
+    return inbox_unit(src, u);
+  }
+  __device__ __forceinline__ void publish_qne() const {
+    reinterpret_cast<uint8_t*>(d.lqm + g)[r] = (uint8_t)qne;   // (little endian: byte r holds bits 8r..8r+7)
+  }
+  // A delivery that skips the cut senders: the Messages of their mail addressed to me go to the back of the link's queue
+  // while it holds fewer than JR_LINK_QUEUE_MSGS.  Whole mailboxes are scanned (the delivery index leaves out no-op
+  // HeartbeatResponses, which count too); an AppendEntries that points at an earlier run is stored with its blocks.
+  __device__ __forceinline__ void queue_cut_mail() {
+    for (uint32_t s_ = 0; s_ < (uint32_t)R; ++s_) {
+      const uint32_t cnt = ((cut >> s_) & 1u) ? L.cin[s_ * 32 + L.lane] : 0u;
+      if (!cnt) continue;
+      const size_t ci = lq_count_at(s_);
+      const uint32_t qc = d.lqc[ci];
+      uint32_t nm = qc & 255u, nu = qc >> 8;
+      for (uint32_t u = 0; u < cnt && nm < JR_LINK_QUEUE_MSGS;) {
+        uint4 h = inbox_unit(s_, u);
+        const uint32_t kind = h.x & 15u, flag = (h.x >> 4) & 1u, aux = (h.x >> 8) & 255u, to = h.x >> 16;
+        const bool ae = kind == JR_CMD_APPEND_ENTRIES;
+        const uint32_t at = (ae && flag) ? h.w : u + 1u;   // the AppendEntries' blocks
+        u += 1u + ((ae && !flag) ? aux : 0u);
+        if (to != TO_PEERS && to != id()) continue;
+        uint32_t take = 1u;
+        if (kind == JR_CMD_VOTE_REQUEST && aux > 1u) {   // aux copies, each a Message: keep the ones that fit
+          take = min(aux, JR_LINK_QUEUE_MSGS - nm);
+          h.x = (h.x & ~(255u << 8)) | (take << 8);
+        }
+        if (ae) h.x &= ~(1u << 4);                      // blocks inline from here on
+        *lq_unit(s_, nu++) = h;
+        if (ae)
+          for (uint32_t k = 0; k < aux; ++k) *lq_unit(s_, nu++) = inbox_unit(s_, at + k);
+        nm += take;
+      }
+      if (nm != (qc & 255u)) {
+        d.lqc[ci] = nm | (nu << 8);
+        qne |= 1u << s_;
+      }
+    }
+    publish_qne();
+  }
+  // End of a delivering tick: the queues of the links that are up were replayed (or lost, if I am silenced or faulted).
+  __device__ __forceinline__ void queue_drop_replayed() {
+    const uint32_t up = qne & ~cut;
+    for (uint32_t s_ = 0; s_ < (uint32_t)R; ++s_)
+      if ((up >> s_) & 1u) d.lqc[lq_count_at(s_)] = 0u;
+    qne &= cut;
+    publish_qne();
+  }
 
   __device__ __forceinline__ void mark(uint32_t to, uint32_t slot) {
     const uint32_t bit = slot < MK_SLOTS ? (1u << slot) : MK_SCAN;
@@ -782,7 +852,7 @@ struct Replica {
       next = (uint32_t)c.host_msg->blocks[k].next;
       tok = c.host_msg->blocks[k].data;
     } else {
-      uint4 u = inbox_unit(c.blk_s, c.blk_at + k);
+      uint4 u = mail_unit(c.blk_s, c.blk_at + k);
       bid = u.x; next = u.y; tok = (uint64_t)u.z | ((uint64_t)u.w << 32);
     }
   }
@@ -1114,6 +1184,8 @@ struct Replica {
     uint32_t reps;   // copies of the current VoteRequest unit still to apply ...
     uint32_t rep_at; // ... and its slot (the unit is re-read, so no Cmd has to stay alive)
     uint32_t tail, tail_i;  // trailing schedule entries: see next_tail
+    uint32_t rq;     // QUEUES: senders whose link queue is still to be replayed this tick (before their own mail)
+    uint32_t src;    // QUEUES: where the units of sender s come from: s (its mailbox) or R + s (the link's queue)
   };
 
   // Which senders have mail for me this tick: one shared-memory read per peer, up front.  Every delivery path (leader
@@ -1180,7 +1252,7 @@ struct Replica {
       if (k.reps) {  // another copy of the same VoteRequest broadcast: re-read the unit
         --k.reps;
         at = k.rep_at;
-        h = inbox_unit(k.s, at);
+        h = mail_unit(QUEUES ? k.src : k.s, at);
         again = true;
         break;
       }
@@ -1190,9 +1262,9 @@ struct Replica {
         h = inbox_unit(k.s, at);
         break;
       }
-      if (k.u < k.cnt) {  // scan delivery (the sender's index overflowed)
+      if (k.u < k.cnt) {  // scan delivery (the sender's index overflowed, or a link queue)
         at = k.u;
-        h = inbox_unit(k.s, k.u);
+        h = mail_unit(QUEUES ? k.src : k.s, k.u);
         const uint32_t k0 = h.x & 15u, to = h.x >> 16;
         k.u += 1u + ((k0 == JR_CMD_APPEND_ENTRIES && !((h.x >> 4) & 1u)) ? ((h.x >> 8) & 255u) : 0u);
         if (to != TO_PEERS && to != me) continue;
@@ -1200,6 +1272,16 @@ struct Replica {
       }
       if (!k.pend) return next_tail(k, p, c);  // peers exhausted: proposals, then Tick
       k.s = (uint32_t)__ffs((int)k.pend) - 1u;
+      if constexpr (QUEUES) {
+        if ((k.rq >> k.s) & 1u) {   // the link's queue first, scanned; the sender stays pending for its own mail
+          k.rq &= ~(1u << k.s);
+          k.src = R + k.s;
+          k.u = 0;
+          k.cnt = d.lqc[lq_count_at(k.s)] >> 8;
+          continue;
+        }
+        k.src = k.s;
+      }
       k.pend &= k.pend - 1u;
       k.u = 0; k.cnt = 0;
       const uint32_t m = d.use_index ? L.mk_in[(r * R + k.s) * 32 + L.lane] : MK_SCAN;
@@ -1209,7 +1291,7 @@ struct Replica {
     const uint32_t kind = h.x & 15u, aux = (h.x >> 8) & 255u;
     c.kind = kind; c.flag = (h.x >> 4) & 1u; c.node_id = k.s + 1; c.nblk = aux; c.block = h.w;
     c.term = (uint64_t)h.y | ((uint64_t)h.z << 32); c.last_term = c.term;
-    c.blk_s = k.s;
+    c.blk_s = QUEUES ? k.src : k.s;
     c.blk_at = (kind == JR_CMD_APPEND_ENTRIES && c.flag) ? h.w : at + 1;
     // N-1 identical VoteRequest broadcasts travel as one unit (candidate.rs:30-37)
     if (!again && kind == JR_CMD_VOTE_REQUEST && aux > 1u) { k.reps = aux - 1u; k.rep_at = at; }
@@ -1219,6 +1301,14 @@ struct Replica {
   __device__ __forceinline__ void run_step(const StepParams& p) {
     Pos k;
     plan_tick(k, p);
+    if constexpr (QUEUES) {
+      k.rq = 0; k.src = 0;
+      if (p.phases & PH_DRAIN) {
+        if (cut) queue_cut_mail();
+        k.rq = qne & ~cut;   // links up again with mail queued: replayed in their sender's place
+        k.pend |= k.rq;
+      }
+    }
     Cmd c;
     c.host_msg = nullptr;
     bool more = live();
@@ -1230,7 +1320,7 @@ struct Replica {
         // path below -- ReplicationProgress::advance + Leader::commit, leader.rs:211-219 --
         // without the generic fetch/dispatch.  Senders are taken in ascending order and the
         // drain stops at the first one that does not fit, so delivery order is unchanged.
-        if (d.use_index && k.idx == 0 && k.u >= k.cnt && k.reps == 0) {
+        if (d.use_index && k.idx == 0 && k.u >= k.cnt && k.reps == 0 && (!QUEUES || k.rq == 0)) {   // (not before a replay)
           const uint32_t real = k.pend & ((1u << R) - 1u);
           // all peers' delivery masks, then all candidate units: independent loads, one latency each
           uint32_t m[R], w[R];
@@ -1296,6 +1386,8 @@ struct Replica {
         }
       }
     }
+    if constexpr (QUEUES)
+      if ((p.phases & PH_DRAIN) && (qne & ~cut)) queue_drop_replayed();
   }
 };
 #undef seen

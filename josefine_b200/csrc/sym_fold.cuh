@@ -26,7 +26,8 @@
 //     fsm_flush uses (fsm_enc_push), fed as the Instructions are produced.
 //   * Stream digests (JR_F_STREAM_DIGEST) need every Message in order, which this path never materialises: engines
 //     created with that flag, or with JR_F_SLED_COMMIT_KEY_STRICT / JR_F_NO_SYMMETRIC_FOLD, never take it.  Nor does a
-//     group with a cut peer link (JR_F_PEER_LINKS): the canonical mail assumes every link delivers.
+//     group with a cut peer link (JR_F_PEER_LINKS): the canonical mail assumes every link delivers; nor one with mail
+//     queued on a link (JR_F_LINK_QUEUES), which its next delivery replays.
 //     tests/test_sym_fold.py compares folded runs with step_kernel runs and with the oracle through everything else:
 //     replica state, block tables, leader tables, Instruction streams -- scenario by scenario and over random scripts.
 //     tests/test_sym_abort.py constructs aborts at chosen ticks and CTA positions (the host build logs which site fired,
@@ -699,6 +700,7 @@ __global__ void __launch_bounds__(32 * R, sym_check_ctas(R)) sym_check_kernel(co
     p0 = d.p0[i]; p1 = d.p1[i]; p2 = d.p2[i]; mk = d.mk[i]; fc = d.fc[i]; tbase = d.tb[g];
     if (p.phases & PH_DRAIN) cnt = d.oc[prv][i];           // mail in flight (the previous tick's outboxes): PH_DRAIN only
     if (d.links) cuts = d.links[g];                        // JR_F_PEER_LINKS: the fold assumes every link is up
+    if (d.lqm) cuts |= d.lqm[g];                           // JR_F_LINK_QUEUES: ... and no queued mail to replay
   }
   if (cnt > 0) u0 = unit(0);
   if (cnt > 1) u1 = unit(1);

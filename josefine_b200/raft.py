@@ -573,6 +573,16 @@ class RaftApi:
                     "isolate_leaders")
         return v.value
 
+    def link_queues(self, groups: Optional[Sequence[int]] = None):
+        """jr_get_link_queues (F_LINK_QUEUES): an (n, 64) uint8 array, [i, 8*(r-1) + (s-1)] = the Messages queued on
+        link s -> r of groups[i] (None: every group)."""
+        import numpy as np
+        n = self.n_groups if groups is None else len(groups)
+        gs = None if groups is None else (C.c_uint32 * max(n, 1))(*groups)
+        out = (C.c_uint8 * max(64 * n, 1))()
+        self._check(self._fn("get_link_queues")(self._h, gs, C.c_size_t(n), out), "get_link_queues")
+        return np.frombuffer(bytes(out), np.uint8)[:64 * n].reshape(n, 64).copy()
+
 
 def link_cut(n_replicas: int, pairs: Iterable[Tuple[int, int]]) -> int:
     """The link matrix that cuts mail from node s to node r for every (s, r) in `pairs` (one direction each)."""
@@ -666,6 +676,7 @@ def _bind(lib: C.CDLL, p: str):
         "set_links": [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.c_size_t],
         "get_links": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(C.c_uint64)],
         "isolate_leaders": [vp, C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)],
+        "get_link_queues": [vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(C.c_uint8)],
     }
     for name, args in sig.items():
         if not hasattr(lib, p + name):   # an older A/B build (JR_ENGINE_LIB): the call site will fail loudly
